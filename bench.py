@@ -124,7 +124,7 @@ def local_map_queries(k, d, z, rng, cam, W, H):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, gpu):
         self.rows, self.proc, self.gpu = [], None, gpu
@@ -460,7 +460,7 @@ class Workload:
         self.ex = self.exs[0]
         self.streams = [torch.cuda.ExternalStream(e.cuda_stream(), device=self.dev) for e in self.exs]
         self.m_last, self.m_local = ORBmatcher(0.9, True), ORBmatcher(0.8, True)
-        # input pool larger than L2 (126 MB), cycled through the timed steps
+        # input pool larger than L2 (50 MB on H100), cycled through the timed steps
         self.pool_batches = max(2, int(np.ceil(pool_bytes / (self.nimg * self.W * self.H))))
         self.pairs = make_pairs(B * self.pool_batches, self.W, self.H, base=8, sigma=sigma, nrect=nrect)
         self.host_pool = torch.from_numpy(self.pairs.reshape(self.pool_batches, self.nimg, self.H, self.W)).pin_memory()
@@ -696,6 +696,35 @@ class Workload:
         return {"ok": True, "against": "CPU oracle (oracle/), same images and query sets, through orbr_submit / orbr_collect", **checked,
                 "compared": "keypoint records (28 B), descriptors, mvuRight / mvDepth float bits, both match arrays: identical"}
 
+    def dump_batch(self, i, out_dir, max_bytes=64 << 20):
+        """Write what batch i handed back on its handle (call right after i was the last batch run there) as out_dir/<name>.npy:
+        keypoints (x, y, size, angle, response, octave, class_id), descriptor bytes, mvuRight, mvDepth, the last-frame search's match
+        per feature row, the local-map search's match per query, per-image counts and per-frame match counts.  All float32 (every
+        integer here is exact in it).  The per-row arrays shrink to a fixed seeded sample of rows (row_index) if they would pass
+        max_bytes in all."""
+        torch = self.torch
+        k, pb = i % self.NH, i % self.pool_batches
+        torch.cuda.synchronize()
+        n, mono, off, kps, desc = self.exs[k].download(self.nimg)
+        rows = int(off[-1])
+        ur, dep = self.exs[k].stereo_download(rows)
+        nq_loc = int(self.H_LOC[pb]["off"][-1])
+        f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+        per_row = {"keypoints": np.stack([kps[f].astype(np.float32) for f in kps.dtype.names], 1), "descriptors": f32(desc),
+                   "mvuRight": f32(ur), "mvDepth": f32(dep), "last_frame_match": f32(self.d_fm[k][:rows].cpu().numpy())}
+        other = {"keypoints_per_image": f32(n), "mono_index_per_image": f32(mono), "row_offsets": f32(off),
+                 "local_map_match": f32(self.d_match[k][:nq_loc].cpu().numpy()), "nmatches_last_frame": f32(self.d_nm[k][:self.B].cpu().numpy()),
+                 "nmatches_local_map": f32(self.d_nm[k][self.B:].cpu().numpy())}
+        row_bytes = sum(a.nbytes for a in per_row.values()) // max(rows, 1)
+        budget = max_bytes - sum(a.nbytes for a in other.values())
+        if rows * (row_bytes + 4) > budget:
+            sel = np.sort(np.random.default_rng(0).choice(rows, budget // (row_bytes + 4), replace=False))
+            per_row = {name: a[sel] for name, a in per_row.items()}
+            other["row_index"] = f32(sel)
+        os.makedirs(out_dir, exist_ok=True)
+        for name, a in {**per_row, **other}.items():
+            np.save(os.path.join(out_dir, name + ".npy"), a)
+
     def close(self):
         for (k, _, _), g in self.graphs.items():
             self.exs[k].graph_destroy(g)
@@ -862,6 +891,8 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="eager launches instead of CUDA-graph replays in the value leg")
     ap.add_argument("--e2e-repeats", type=int, default=5)
     ap.add_argument("--latency-frames", type=int, default=200)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last batch of the timed steps computed as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -918,6 +949,8 @@ def main():
     t_end = time.time()
     clocks = sampler.stop(t_begin, t_end)
     launches = _native.lib().orb_kernel_launches() - launches0
+    if args.dump_outputs and rank == 0:
+        wl.dump_batch(nwarm + args.steps * BPS - 1, args.dump_outputs)
     ms_max = max_ranks(ms)
     value = world * B * BPS * args.steps / (ms_max * 1e-3)
     nm_host = wl.d_nm[0].cpu().numpy()
@@ -1008,7 +1041,7 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", 3350.0))
         level_px = [ex.level_size(l)[0] * ex.level_size(l)[1] for l in range(8)]
 
         def stage_table(stage, serial, n_kp_, n_cand_):
@@ -1036,7 +1069,7 @@ def main():
             break
         roofline = {"bound": "hbm", "kernel": top, "achieved": achieved, "peak": peak, "unit": "GB/s",
                     "frac": achieved / peak, "traffic": traffic,
-                    "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                    "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "H100 SXM data sheet 3350 GB/s (not measured)",
                     "stage_ms_per_batch": stages, "stage_gbs": gbs, "algorithmic_bytes_per_image": ab,
                     "fast_blur_orient_describe": frb, "traffic_source": tsrc,
                     "images_per_launch": nimg, "fast_candidates_per_image": n_cand,
@@ -1088,7 +1121,7 @@ def main():
                            "timed_region_s": ms_max * 1e-3,
                            "queries_per_frame": {"last_frame": wl.nq_last / B, "local_map": wl.nq_loc / B},
                            "matches_per_frame": {"last_frame": float(nm_host[:B].mean()), "local_map": float(nm_host[B:].mean())},
-                           "l2": f"input pool of {wl.pool_batches} batches = {wl.pool_batches * nimg * W * H / 1e6:.0f} MB > 126 MB L2, "
+                           "l2": f"input pool of {wl.pool_batches} batches = {wl.pool_batches * nimg * W * H / 1e6:.0f} MB > 50 MB L2 (H100), "
                                  "intermediates rewritten every batch",
                            "keypoints_per_image": n_kp, "fast_candidates_per_image": n_cand,
                            "kernel_variants": {"quadtree": int(os.environ.get("ORB_QT_VARIANT", "1") != "0"),

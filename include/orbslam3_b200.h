@@ -1,4 +1,4 @@
-/* orbslam3_b200.h -- C ABI of liborbslam3_b200.so: the B200 (sm_100a) implementation of ORB-SLAM3's
+/* orbslam3_b200.h -- C ABI of liborbslam3_b200.so: the H100 (sm_90a) implementation of ORB-SLAM3's
  * per-frame data-parallel hot path.  Plain pointers and sizes only; every function returns an
  * orb_status (0 = ok, <0 = error) and never throws.  The caller owns all host buffers; the library owns
  * device memory per handle; one CUDA stream per handle; thread-safe across handles, not within one.

@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of ORB-SLAM3's per-frame hot path behind the reference's own
+"""H100-native (sm_90a) implementation of ORB-SLAM3's per-frame hot path behind the reference's own
 ORBextractor / ORBmatcher / Optimizer interfaces.  See DESIGN.md."""
 from ._native import OrbError, build, lib, KP_DTYPE  # noqa: F401
 from .extractor import ORBextractor  # noqa: F401

@@ -14,7 +14,7 @@ _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("ORB_LIB_PATH") or os.path.join(_PKG, "lib", "liborbslam3_b200.so")   # ORB_LIB_PATH: an instrumented build (tools/qt_phases.py)
 SOURCES = ["extractor.cu", "stereo.cu", "matcher.cu", "triangulation.cu", "lba.cu", "poseopt.cu", "bow.cu", "mappoint.cu", "liba.cu", "knn.cu", "replay.cu"]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"),
@@ -26,7 +26,7 @@ class OrbError(RuntimeError):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into lib/liborbslam3_b200.so (nvcc cross-compiles on CPU)."""
+    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so (nvcc cross-compiles on CPU)."""
     srcs = [os.path.join(_CSRC, s) for s in SOURCES]
     deps = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)] + [os.path.join(_PKG, "..", "include", "orbslam3_b200.h")]
     if os.environ.get("ORB_LIB_PATH"):

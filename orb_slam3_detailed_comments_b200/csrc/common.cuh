@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations of the sm_100a hot-path library (liborbslam3_b200.so)
+// common.cuh -- shared declarations of the sm_90a hot-path library (liborbslam3_b200.so)
 #pragma once
 #include <utility>
 #include <cstdlib>
@@ -56,6 +56,33 @@ inline cudaError_t launch_p(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
     at[0].val.priority = launch_priority();
     cfg.attrs = at; cfg.numAttrs = launch_priority() != 0 ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+}
+
+inline int device_sm_count(int device) {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device);
+    return n > 0 ? n : 1;
+}
+
+// Halve a thread-block cluster size (*cs) until the device can co-schedule one cluster of `kern` with this block and dynamic shared
+// memory: a 16-CTA (non-portable) cluster needs 16 SMs with room for the block inside one GPC, which not every H100 GPC has.  A
+// failing query is returned as the error it is, never taken for "does not fit".
+template <typename... KArgs>
+inline cudaError_t fit_cluster_size(void (*kern)(KArgs...), int* cs, int threads, size_t smem) {
+    while (*cs > 1) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(*cs); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = *cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        cfg.attrs = at; cfg.numAttrs = 1;
+        int n = 0;
+        const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
+        if (e != cudaSuccess) return e;
+        if (n > 0) break;
+        *cs >>= 1;
+    }
+    return cudaSuccess;
 }
 
 #define ORB_MAX_LEVELS 12

@@ -1,6 +1,6 @@
-// devmath.cuh -- per-element arithmetic of the ORB hot path, written once for the sm_100a kernels.
+// devmath.cuh -- per-element arithmetic of the ORB hot path, written once for the sm_90a kernels.
 // Every function is ORB_HD so that tests/host_emul can compile this header with g++ (no GPU in the
-// build container) and compare it against the oracle before a kernel ever runs on a B200.
+// build container) and compare it against the oracle before a kernel ever runs on the GPU.
 #pragma once
 #include <stdint.h>
 

@@ -1,4 +1,4 @@
-// extractor_kernels.cuh -- sm_100a kernels of ORBextractor::operator()
+// extractor_kernels.cuh -- sm_90a kernels of ORBextractor::operator()
 // (/root/reference/src/ORBextractor.cc:1557-1682).  All kernels are batched: blockIdx.{y|z} or a
 // division of blockIdx.x selects the image, so one launch covers a whole batch of frames.
 #pragma once
@@ -428,7 +428,7 @@ __global__ void __launch_bounds__(QT_THREADS) k_quadtree(const __grid_constant__
 
 // K3 variant 1: the candidate sort takes up to three butterfly stages per pass, and the ordered phase's std::sort is spread over the CTA
 // instead of run by thread 0 (both in quadtree_sort_par.cuh).  A separate
-// kernel so that k_quadtree -- green on a B200 in round 1 -- keeps its machine code bit for bit (scripts/sass_fingerprint.py);
+// kernel so that k_quadtree -- green on the GPU tier -- keeps its machine code bit for bit (scripts/sass_fingerprint.py);
 // selected with ORB_QT_VARIANT=1 at orbx_create until it has had its own device run.
 __device__ __forceinline__ int qt_run_v1(uint32_t* arr, void* ws, int cap, int n, int npow, const uint32_t* __restrict__ src,
                                          const QtGeom& q, uint32_t* out) {
@@ -573,9 +573,9 @@ __device__ __forceinline__ int reflect101(int i, int n) {
 // lo = (px0 | px2 << 16), hi = (px1 | px3 << 16)
 // mode 0: interior (three aligned word loads); mode 1: left edge, x0 == 0 (columns -3 .. -1 reflect to 3 .. 1: one PRMT of the first
 // word); mode 2: right edge: ten byte loads, window column x0 - 3 + k read at itself while k < kr and at its mirror image
-// 2w - 2 - column from there on (BORDER_REFLECT_101; columns past w + 2 only feed the pitch padding).  ncu, round 2: with the reflect
-// arithmetic inside the row loop the edge path was 35 % of k_blur's instructions -- a warp that holds one edge lane runs it for
-// every row (profiles/r02_source_lines.md).
+// 2w - 2 - column from there on (BORDER_REFLECT_101; columns past w + 2 only feed the pitch padding).  With the reflect
+// arithmetic inside the row loop the edge path was a large share of k_blur's instructions -- a warp that holds one edge lane runs it for
+// every row.
 template <bool DP4A>
 __device__ __forceinline__ void blur_h4(const uint8_t* __restrict__ p, int x0, int mode, int kr, int colA, int colB, uint32_t* __restrict__ h) {
     uint32_t w0, w1, w2;   // bytes x0-4 .. x0+7
@@ -675,7 +675,7 @@ __global__ void __launch_bounds__(OD_WARPS * 32) k_orient_describe(const __grid_
                                                                   orbx_keypoint* __restrict__ kps, uint8_t* __restrict__ desc) {
     // patT: the 256 point pairs as one 32-bit word each (xa, ya, xb, yb as int8), transposed so that lane's k-th pair sits at
     // [k][lane] -- built once per handle in global memory.  (Round 1 staged it per CTA from __constant__ memory: 32 different constant
-    // addresses per load serialise, and the staging + barrier were 25 % of the kernel's stall samples, profiles/r02_source_lines.md.)
+    // addresses per load serialise, and the staging + barrier were a large share of the kernel's stall samples.)
     const int img = blockIdx.y;
     const int lane = threadIdx.x & 31;
     const int e = blockIdx.x * OD_WARPS + (threadIdx.x >> 5);

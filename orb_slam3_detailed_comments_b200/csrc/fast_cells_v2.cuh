@@ -2,7 +2,7 @@
 // (ORBextractor.cc:1069-1166; cv::FAST(cell, thr, nms = true) per 35-px cell, SURVEY App. A.3).
 //
 // Same result as k_fast_cells (the candidate list of a level is order-free: the quadtree re-derives the reference order from the
-// coordinates), about half the instructions.  What changed, each from the round-1 ncu source page (profiles/r01_source_lines.md):
+// coordinates), about half the instructions.  What changed, each from an ncu source page of k_fast_cells:
 //   * the cell geometry comes from a host-built table (one 8-byte record per NON-EMPTY cell) instead of a per-CTA level search,
 //     two integer divisions and the bounds logic;
 //   * the window is staged 8 pixels per step (one 64-bit load, two 128-bit shared stores) into rows sized from the geometry

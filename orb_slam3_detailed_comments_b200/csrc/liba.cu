@@ -2,7 +2,6 @@
 // The algorithm lives in liba_core.cuh as barrier-separated SPMD phases shared with the CPU emulation harness; this file is
 // the launch wrapper: one thread-block cluster (or one CTA) per window, everything for a window in one blob (liba_pack.h),
 // fp64 throughout.
-// STATUS: cross-compiles for sm_100a and is validated on the host through tests/host_emul; first GPU run is pending.
 #include <cuda_runtime.h>
 #include <stdlib.h>
 
@@ -43,6 +42,7 @@ struct liba_handle {
     size_t d_bytes = 0;
     uint8_t* h_buf = nullptr;
     size_t h_bytes = 0;
+    int n_sms = 1;
 };
 
 extern "C" orb_status liba_create(int32_t device, liba_handle** out) {
@@ -54,6 +54,7 @@ extern "C" orb_status liba_create(int32_t device, liba_handle** out) {
     ORB_CUDA(cudaSetDevice(device));
     liba_handle* h = new liba_handle();
     h->device = device;
+    h->n_sms = device_sm_count(device);
     if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
         delete h;
         return set_error(ORB_ERR_CUDA, "cudaStreamCreate failed");
@@ -119,11 +120,13 @@ extern "C" orb_status liba_solve(liba_handle* h, int32_t n_problems, const liba_
         ORB_CUDA(cudaMemcpyAsync(h->d_buf + base[i], h->h_buf + base[i], lay[i].io_bytes + lay[i].in_bytes, cudaMemcpyHostToDevice, h->stream));
     // one or two windows get a cluster of 16 SMs each (the non-portable size), small batches 8, large ones fewer
     // (ORB_LIBA_CLUSTER = 1 | 2 | 4 | 8 | 16 overrides: a tuning knob)
-    int cs = n_problems <= 2 ? 16 : ((n_problems * LIBA_CS_MAX <= 148) ? LIBA_CS_MAX : (n_problems * 4 <= 148 ? 4 : (n_problems * 2 <= 148 ? 2 : 1)));
+    const int sms = h->n_sms;
+    int cs = n_problems <= 2 ? 16 : ((n_problems * LIBA_CS_MAX <= sms) ? LIBA_CS_MAX : (n_problems * 4 <= sms ? 4 : (n_problems * 2 <= sms ? 2 : 1)));
     if (const char* e = getenv("ORB_LIBA_CLUSTER")) {
         const int v = atoi(e);
         if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) cs = v;
     }
+    ORB_CUDA(fit_cluster_size(k_liba, &cs, LIBA_THREADS, 0));
     {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(n_problems * cs);

@@ -408,7 +408,7 @@ ORB_HD void qt_bitonic_sort_r8(uint32_t* arr, int npow) {
 
 #if defined(__CUDACC__)
 // ---- device only: bitonic sort whose strides <= 128 never touch shared memory -----------------------------------------------
-// ncu (round 2, profiles/r02_source_lines.md): qt_bitonic_sort_r8 spent 26 % (level 0) / 43 % (levels 1-7) of k_quadtree_v1 and four
+// Under ncu qt_bitonic_sort_r8 was a large share of k_quadtree_v1 (the larger at levels 1-7) and took four
 // times the ideal shared-memory wavefronts -- in the passes with strides < 32 a thread's eight elements are 8 / 4 / 2 words apart
 // from its neighbour's, an 8- / 4- / 2-way bank conflict on all sixteen accesses.  Here a warp owns 256 consecutive elements: lane
 // i holds arr[base + 4 i .. + 3] and arr[base + 128 + 4 i .. + 3] (two conflict-free 128-bit accesses), so strides 128, 2 and 1 are

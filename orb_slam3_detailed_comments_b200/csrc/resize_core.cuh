@@ -2,8 +2,8 @@
 // fixed-point model (ORBextractor.cc:1687-1738, SURVEY App. A.1), written so that the identical source runs as a device function and
 // on the host (tests/host_emul, against the oracle's resize).
 //
-// k_resize_v2 spends 40 % of its instructions and two thirds of its stall samples on the eight byte loads of a source row
-// (profiles/r02_source_lines_final.md).  Here a source row's bytes x0 .. x0 + 7 (x0 = the first tap of the thread's first pixel) are
+// k_resize_v2 spends a large share of its instructions and most of its stall samples on the eight byte loads of a source row
+// (ncu source page).  Here a source row's bytes x0 .. x0 + 7 (x0 = the first tap of the thread's first pixel) are
 // three aligned word loads and two funnel shifts; pixel i's tap pair (p[x0_i], p[x0_i + 1]) is one PRMT with a per-thread selector,
 // and c0 * p0 + c1 * p1 is ONE IDP.2A: the 11-bit coefficients are the two 16-bit operands, the pixels the two byte operands.
 // The clamped tap x1 = min(x0 + 1, w - 1) differs from x0 + 1 only where the table has c1 = 0, so the product is the same.

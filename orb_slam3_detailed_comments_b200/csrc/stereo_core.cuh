@@ -42,7 +42,7 @@ ORB_HD uint32_t st_funnel(uint32_t lo, uint32_t hi, uint32_t sh) {
     return sh ? (lo >> sh) | (hi << (32u - sh)) : lo;
 #endif
 }
-// acc + sum of |a_i - b_i| over the four bytes (VABSDIFF4.U8 with accumulate: one instruction on sm_100a)
+// acc + sum of |a_i - b_i| over the four bytes (VABSDIFF4.U8 with accumulate: one instruction on sm_90a)
 ORB_HD uint32_t st_sad4(uint32_t a, uint32_t b, uint32_t acc) {
 #if defined(__CUDA_ARCH__)
     uint32_t d;

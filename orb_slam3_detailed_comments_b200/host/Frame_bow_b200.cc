@@ -1,4 +1,4 @@
-// Frame_bow_b200.cc -- Frame::ComputeBoW (/root/reference/src/Frame.cc:984-997) on the B200.
+// Frame_bow_b200.cc -- Frame::ComputeBoW (/root/reference/src/Frame.cc:984-997) on the GPU.
 //
 // Compiled against the reference's headers.  mpORBvocabulary->transform(descriptors, mBowVec, mFeatVec, 4) -- DBoW2's tree walk of every
 // descriptor, TF-IDF weights, the L1-normalised BowVector and the level-4 FeatureVector -- is orbv_transform over the descriptors the
@@ -65,9 +65,9 @@ namespace ORB_SLAM3 {
 
 void Frame::ComputeBoW() {
     if (!mBowVec.empty()) return;
-    if (Nleft != -1) throw orb_b200::Error("Frame::ComputeBoW: Nleft != -1 (fisheye stereo rig) is not built on the B200 path");
+    if (Nleft != -1) throw orb_b200::Error("Frame::ComputeBoW: Nleft != -1 (fisheye stereo rig) is not built on the GPU path");
     orbx_handle* h = orb_b200_handle_of(mpORBextractorLeft);
-    if (!h) throw orb_b200::Error("Frame::ComputeBoW: the frame's extractor is not a B200 extractor");
+    if (!h) throw orb_b200::Error("Frame::ComputeBoW: the frame's extractor is not a GPU-path extractor");
     int32_t n = 0;
     orb_b200::check(orbx_counts(h, &n, nullptr, nullptr), "orbx_counts");
     if (n != N) throw orb_b200::Error("Frame::ComputeBoW: the frame is not the one its extractor produced last");

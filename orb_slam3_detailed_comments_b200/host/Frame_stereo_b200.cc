@@ -1,4 +1,4 @@
-// Frame_stereo_b200.cc -- Frame::ComputeStereoMatches (/root/reference/src/Frame.cc:1102-1358) on the B200.
+// Frame_stereo_b200.cc -- Frame::ComputeStereoMatches (/root/reference/src/Frame.cc:1102-1358) on the GPU.
 //
 // Replaces that one member of the reference's Frame.cc (compile Frame.cc with the member's body excluded, or link this object
 // first with -Wl,--allow-multiple-definition; INTEGRATION.md).  Both extractor objects of the frame are ours
@@ -17,7 +17,7 @@ void Frame::ComputeStereoMatches() {
     mvDepth = std::vector<float>(N, -1.0f);
     orbx_handle* hl = orb_b200_handle_of(mpORBextractorLeft);
     orbx_handle* hr = orb_b200_handle_of(mpORBextractorRight);
-    if (!hl || !hr) throw orb_b200::Error("Frame::ComputeStereoMatches: the frame's extractors are not B200 extractors");
+    if (!hl || !hr) throw orb_b200::Error("Frame::ComputeStereoMatches: the frame's extractors are not GPU-path extractors");
     if (N == 0) return;
     orb_b200::check(orbm_stereo_pair(hl, hr, mbf, mb, mvuRight.data(), mvDepth.data(), N), "orbm_stereo_pair");
 }

@@ -3,7 +3,7 @@
 // Compiled AGAINST THE REFERENCE'S OWN HEADER (include/ORBextractor.h, unchanged) and linked with
 // liborbslam3_b200.so instead of the reference's ORBextractor.cc, it gives Tracking / Frame the same
 // ORB_SLAM3::ORBextractor class: same constructor, same operator(), same getters, mvImagePyramid populated.
-// All arithmetic happens on the B200 behind the C ABI (include/orbslam3_b200.h); this file only marshals.
+// All arithmetic happens on the GPU behind the C ABI (include/orbslam3_b200.h); this file only marshals.
 //
 //   g++ -std=c++14 -I<ORB_SLAM3>/include -I<this repo>/include $(pkg-config --cflags opencv4) \
 //       -c ORBextractor_b200.cc            # then link -lorbslam3_b200 in place of ORBextractor.o

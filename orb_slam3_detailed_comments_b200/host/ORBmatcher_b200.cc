@@ -1,4 +1,4 @@
-// ORBmatcher_b200.cc -- the per-frame members of ORB_SLAM3::ORBmatcher (/root/reference/src/ORBmatcher.cc) on the B200.
+// ORBmatcher_b200.cc -- the per-frame members of ORB_SLAM3::ORBmatcher (/root/reference/src/ORBmatcher.cc) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/ORBmatcher.h.  Provides the constructor, the three static constants,
 // DescriptorDistance and the two searches the tracking thread runs on every frame:
@@ -9,7 +9,7 @@
 // of INTEGRATION.md (every one of them has a kernel: orbm_search_keyframe, orbm_search_bow*, orbm_search_triangulation, ...).
 //
 // Both searches read the frame's keypoints, descriptors, mvuRight and grid from the DEVICE: the frame searched is the frame the
-// B200 extractor behind F.mpORBextractorLeft produced last (true at both call sites: the current frame), so nothing but the
+// GPU-path extractor behind F.mpORBextractorLeft produced last (true at both call sites: the current frame), so nothing but the
 // query side (a few KB per call) is uploaded.  Only marshaling happens here; Nleft != -1 rigs (fisheye pairs) are not built.
 #include <cmath>
 #include <cstring>
@@ -45,9 +45,9 @@ orbm_camera camera_of(const Frame& F) {
     return c;
 }
 orbx_handle* device_frame(const Frame& F, const char* who) {
-    if (F.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the B200 path");
+    if (F.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the GPU path");
     orbx_handle* h = orb_b200_handle_of(F.mpORBextractorLeft);
-    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a B200 extractor");
+    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a GPU-path extractor");
     int32_t n = 0;
     orb_b200::check(orbx_counts(h, &n, nullptr, nullptr), "orbx_counts");
     if (n != F.N) throw orb_b200::Error(std::string(who) + ": the frame is not the one its extractor produced last");

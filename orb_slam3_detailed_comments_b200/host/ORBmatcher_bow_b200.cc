@@ -1,4 +1,4 @@
-// ORBmatcher_bow_b200.cc -- the two bag-of-words searches of ORB_SLAM3::ORBmatcher (/root/reference/src/ORBmatcher.cc) on the B200.
+// ORBmatcher_bow_b200.cc -- the two bag-of-words searches of ORB_SLAM3::ORBmatcher (/root/reference/src/ORBmatcher.cc) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/ORBmatcher.h, next to ORBmatcher_b200.cc (constructor, constants, the per-frame
 // projection searches):
@@ -33,7 +33,7 @@ struct QuerySide {            // the keyframe whose map points are looked for
 };
 
 QuerySide query_side(KeyFrame* pKF, const std::vector<MapPoint*>& vpMapPointsKF, const char* who) {
-    if (pKF->mpCamera2 || pKF->NLeft != -1) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the B200 path");
+    if (pKF->mpCamera2 || pKF->NLeft != -1) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the GPU path");
     QuerySide q;
     for (DBoW2::FeatureVector::const_iterator it = pKF->mFeatVec.begin(); it != pKF->mFeatVec.end(); ++it)
         for (size_t k = 0; k < it->second.size(); ++k) {
@@ -63,9 +63,9 @@ std::vector<int32_t> node_of_features(const DBoW2::FeatureVector& fv, int N) {  
 // ORBmatcher.cc:259-493
 int ORBmatcher::SearchByBoW(KeyFrame* pKF, Frame& F, std::vector<MapPoint*>& vpMapPointMatches) {
     const char* who = "ORBmatcher::SearchByBoW(KeyFrame*, Frame&)";
-    if (F.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the B200 path");
+    if (F.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the GPU path");
     orbx_handle* h = orb_b200_handle_of(F.mpORBextractorLeft);
-    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a B200 extractor");
+    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a GPU-path extractor");
     int32_t n = 0;
     orb_b200::check(orbx_counts(h, &n, nullptr, nullptr), "orbx_counts");
     if (n != F.N) throw orb_b200::Error(std::string(who) + ": the frame is not the one its extractor produced last");
@@ -94,7 +94,7 @@ int ORBmatcher::SearchByBoW(KeyFrame* pKF1, KeyFrame* pKF2, std::vector<MapPoint
     const std::vector<MapPoint*> vpMapPoints1 = pKF1->GetMapPointMatches(), vpMapPoints2 = pKF2->GetMapPointMatches();
     vpMatches12 = std::vector<MapPoint*>(vpMapPoints1.size(), static_cast<MapPoint*>(NULL));
     const QuerySide Q = query_side(pKF1, vpMapPoints1, who);
-    if (pKF2->mpCamera2 || pKF2->NLeft != -1) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the B200 path");
+    if (pKF2->mpCamera2 || pKF2->NLeft != -1) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the GPU path");
     const int nq = (int)Q.src.size(), n2 = (int)vpMapPoints2.size();
     if (nq == 0 || n2 == 0) return 0;
     std::vector<orbx_keypoint> kp2(n2);

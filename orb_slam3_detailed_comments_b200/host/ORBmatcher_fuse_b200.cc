@@ -1,5 +1,5 @@
 // ORBmatcher_fuse_b200.cc -- ORBmatcher::Fuse(KeyFrame*, const vector<MapPoint*>&, th, bRight) (/root/reference/src/ORBmatcher.cc:1325-1544)
-// on the B200.
+// on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/ORBmatcher.h.  LocalMapping::SearchInNeighbors runs it twice per neighbour for every
 // new keyframe (LocalMapping.cc:703, 746).  On the host: the caller-side skips (NULL, isBad(), IsInKeyFrame), the query arrays, and the
@@ -29,7 +29,7 @@ namespace ORB_SLAM3 {
 
 int ORBmatcher::Fuse(KeyFrame* pKF, const std::vector<MapPoint*>& vpMapPoints, const float th, const bool bRight) {
     const char* who = "ORBmatcher::Fuse(KeyFrame*, vpMapPoints)";
-    if (bRight || pKF->mpCamera2) throw orb_b200::Error(std::string(who) + ": the second camera of a rig is not built on the B200 path");
+    if (bRight || pKF->mpCamera2) throw orb_b200::Error(std::string(who) + ": the second camera of a rig is not built on the GPU path");
     orbx_handle* h = orb_b200_keyframe_search_handle();
     if (!h) throw orb_b200::Error(std::string(who) + ": no device workspace yet (orb_b200_use_handle_for_keyframe_searches)");
     const int nMPs = (int)vpMapPoints.size();

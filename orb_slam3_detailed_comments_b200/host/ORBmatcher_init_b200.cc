@@ -1,4 +1,4 @@
-// ORBmatcher_init_b200.cc -- ORBmatcher::SearchForInitialization (/root/reference/src/ORBmatcher.cc:734-890) on the B200.
+// ORBmatcher_init_b200.cc -- ORBmatcher::SearchForInitialization (/root/reference/src/ORBmatcher.cc:734-890) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/ORBmatcher.h.  Monocular initialisation (Tracking.cc:2588) runs it on every frame
 // until a map exists: the reference frame F1 (host memory) against the current frame F2, which is the frame its extractor produced last
@@ -16,9 +16,9 @@ namespace ORB_SLAM3 {
 
 int ORBmatcher::SearchForInitialization(Frame& F1, Frame& F2, std::vector<cv::Point2f>& vbPrevMatched, std::vector<int>& vnMatches12, int windowSize) {
     const char* who = "ORBmatcher::SearchForInitialization";
-    if (F1.Nleft != -1 || F2.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the B200 path");
+    if (F1.Nleft != -1 || F2.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the GPU path");
     orbx_handle* h = orb_b200_handle_of(F2.mpORBextractorLeft);
-    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a B200 extractor");
+    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a GPU-path extractor");
     const int n1 = (int)F1.mvKeysUn.size(), n2 = (int)F2.mvKeysUn.size();
     vnMatches12 = std::vector<int>(n1, -1);
     if (n1 == 0 || n2 == 0) return 0;

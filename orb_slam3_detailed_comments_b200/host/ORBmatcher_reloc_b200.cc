@@ -1,5 +1,5 @@
 // ORBmatcher_reloc_b200.cc -- ORBmatcher::SearchByProjection(Frame& CurrentFrame, KeyFrame* pKF, const set<MapPoint*>& sAlreadyFound, th, ORBdist)
-// (/root/reference/src/ORBmatcher.cc:2196-2330) on the B200.
+// (/root/reference/src/ORBmatcher.cc:2196-2330) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/ORBmatcher.h.  Tracking::Relocalization runs it after the first PnP inliers to pick up
 // the candidate keyframe's remaining map points (Tracking.cc:3758, 3773).  On the host: the queries -- the keyframe's good map points that are
@@ -26,9 +26,9 @@ namespace ORB_SLAM3 {
 
 int ORBmatcher::SearchByProjection(Frame& CurrentFrame, KeyFrame* pKF, const std::set<MapPoint*>& sAlreadyFound, const float th, const int ORBdist) {
     const char* who = "ORBmatcher::SearchByProjection(CurrentFrame, pKF, sAlreadyFound)";
-    if (CurrentFrame.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the B200 path");
+    if (CurrentFrame.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the GPU path");
     orbx_handle* h = orb_b200_handle_of(CurrentFrame.mpORBextractorLeft);
-    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a B200 extractor");
+    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a GPU-path extractor");
     int32_t n = 0;
     orb_b200::check(orbx_counts(h, &n, nullptr, nullptr), "orbx_counts");
     if (n != CurrentFrame.N) throw orb_b200::Error(std::string(who) + ": the frame is not the one its extractor produced last");

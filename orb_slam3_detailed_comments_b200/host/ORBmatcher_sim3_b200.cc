@@ -1,5 +1,5 @@
 // ORBmatcher_sim3_b200.cc -- the loop-closing / map-merging searches that project map points into a keyframe through a Sim3 pose
-// (/root/reference/src/ORBmatcher.cc) on the B200:
+// (/root/reference/src/ORBmatcher.cc) on the GPU:
 //   SearchByProjection(KeyFrame* pKF, Sophus::Sim3f& Scw, const vector<MapPoint*>& vpPoints, vector<MapPoint*>& vpMatched, int th, float ratioHamming)   :495-618
 //   the overload with vpPointsKFs / vpMatchedKF                                                                                                        :620-732
 //   Fuse(KeyFrame* pKF, Sophus::Sim3f& Scw, const vector<MapPoint*>& vpPoints, float th, vector<MapPoint*>& vpReplacePoint)                               :1546-1687
@@ -34,7 +34,7 @@ struct Sim3Search {
 Sim3Search search(ORB_SLAM3::KeyFrame* pKF, Sophus::Sim3f& Scw, const std::vector<ORB_SLAM3::MapPoint*>& vpPoints, const std::set<ORB_SLAM3::MapPoint*>& skip,
                   const uint8_t* feat_claimed, int variant, float th, float hamming_max, bool checkOri, const char* who) {
     using namespace ORB_SLAM3;
-    if (pKF->mpCamera2) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the B200 path");
+    if (pKF->mpCamera2) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the GPU path");
     orbx_handle* h = orb_b200_keyframe_search_handle();
     if (!h) throw orb_b200::Error(std::string(who) + ": no device workspace yet (orb_b200_use_handle_for_keyframe_searches)");
     const Sophus::SE3f Tcw = Sophus::SE3f(Scw.rotationMatrix(), Scw.translation() / Scw.scale());

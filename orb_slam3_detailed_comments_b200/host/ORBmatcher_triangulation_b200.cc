@@ -1,4 +1,4 @@
-// ORBmatcher_triangulation_b200.cc -- ORBmatcher::SearchForTriangulation (/root/reference/src/ORBmatcher.cc:1045-1323) on the B200.
+// ORBmatcher_triangulation_b200.cc -- ORBmatcher::SearchForTriangulation (/root/reference/src/ORBmatcher.cc:1045-1323) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/ORBmatcher.h.  LocalMapping::CreateNewMapPoints runs it for every new keyframe
 // against its best covisible neighbours (LocalMapping.cc:379).  On the host: the relative pose, the epipole and the fundamental matrix in
@@ -29,7 +29,7 @@ void put_keypoint(orbx_keypoint& o, const cv::KeyPoint& k) {
 int ORBmatcher::SearchForTriangulation(KeyFrame* pKF1, KeyFrame* pKF2, std::vector<std::pair<size_t, size_t> >& vMatchedPairs, const bool bOnlyStereo,
                                        const bool bCoarse) {
     const char* who = "ORBmatcher::SearchForTriangulation";
-    if (pKF1->mpCamera2 || pKF2->mpCamera2) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the B200 path");
+    if (pKF1->mpCamera2 || pKF2->mpCamera2) throw orb_b200::Error(std::string(who) + ": a keyframe with a second camera is not built on the GPU path");
     orbx_handle* h = orb_b200_keyframe_search_handle();
     if (!h) throw orb_b200::Error(std::string(who) + ": no device workspace yet (orb_b200_use_handle_for_keyframe_searches)");
 

@@ -1,4 +1,4 @@
-// Optimizer_lba_b200.cc -- Optimizer::LocalBundleAdjustment (/root/reference/src/Optimizer.cc:1740-2188) on the B200.
+// Optimizer_lba_b200.cc -- Optimizer::LocalBundleAdjustment (/root/reference/src/Optimizer.cc:1740-2188) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/Optimizer.h (signature :59).  What stays on the host is what touches the
 // map's objects: choosing the local window (:1744-1855), flattening it into the SoA problem the solver takes (:1873-2091),
@@ -94,7 +94,7 @@ void Optimizer::LocalBundleAdjustment(KeyFrame* pKF, bool* pbStopFlag, Map* pMap
         for (const auto& ob : vObs[p]) {
             KeyFrame* pKFi = ob.first;
             if (pKFi->isBad() || pKFi->GetMap() != pCurrentMap) continue;
-            if (pKFi->mpCamera2) throw orb_b200::Error("LocalBundleAdjustment: a keyframe with a second camera (EdgeSE3ProjectXYZToBody) is not built on the B200 path");
+            if (pKFi->mpCamera2) throw orb_b200::Error("LocalBundleAdjustment: a keyframe with a second camera (EdgeSE3ProjectXYZToBody) is not built on the GPU path");
             const int leftIndex = std::get<0>(ob.second);
             if (leftIndex == -1) continue;
             const auto it = kfIndex.find(pKFi);

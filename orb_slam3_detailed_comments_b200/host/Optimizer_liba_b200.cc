@@ -1,4 +1,4 @@
-// Optimizer_liba_b200.cc -- Optimizer::LocalInertialBA (/root/reference/src/Optimizer.cc:2203-2812) on the B200.
+// Optimizer_liba_b200.cc -- Optimizer::LocalInertialBA (/root/reference/src/Optimizer.cc:2203-2812) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/Optimizer.h (signature :86).  What stays on the host is what touches the map's
 // objects: the temporal window (the keyframe and its mPrevKF chain, :2217-2245), its map points (:2248-2270), the fixed keyframes
@@ -134,7 +134,7 @@ void Optimizer::LocalInertialBA(KeyFrame* pKF, bool* pbStopFlag, Map* pMap, int&
             const Eigen::Vector3d v = k->GetVelocity().cast<double>(), bg = k->GetGyroBias().cast<double>(), ba = k->GetAccBias().cast<double>();
             for (int c = 0; c < 3; ++c) { S[12 + c] = v(c); S[15 + c] = bg(c); S[18 + c] = ba(c); }
         } else if (!isFixed) {
-            throw orb_b200::Error("LocalInertialBA: an optimisable keyframe without IMU (bImu false) is not built on the B200 path");
+            throw orb_b200::Error("LocalInertialBA: an optimisable keyframe without IMU (bImu false) is not built on the GPU path");
         }
         const Sophus::SE3f Tk = k->mImuCalib.mTcb;
         for (int r = 0; r < 3; ++r) {
@@ -182,7 +182,7 @@ void Optimizer::LocalInertialBA(KeyFrame* pKF, bool* pbStopFlag, Map* pMap, int&
             KeyFrame* pKFi = ob.first;
             if (pKFi->mnBALocalForKF != ba_id && pKFi->mnBAFixedForKF != ba_id) continue;
             if (pKFi->isBad() || pKFi->GetMap() != pCurrentMap) continue;
-            if (pKFi->mpCamera2) throw orb_b200::Error("LocalInertialBA: a keyframe with a second camera (EdgeMono(1)) is not built on the B200 path");
+            if (pKFi->mpCamera2) throw orb_b200::Error("LocalInertialBA: a keyframe with a second camera (EdgeMono(1)) is not built on the GPU path");
             const int leftIndex = std::get<0>(ob.second);
             if (leftIndex == -1) continue;
             const auto it = kfIndex.find(pKFi);

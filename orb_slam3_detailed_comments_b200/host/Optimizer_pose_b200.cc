@@ -1,4 +1,4 @@
-// Optimizer_pose_b200.cc -- Optimizer::PoseOptimization(Frame*) (/root/reference/src/Optimizer.cc:55-412) on the B200.
+// Optimizer_pose_b200.cc -- Optimizer::PoseOptimization(Frame*) (/root/reference/src/Optimizer.cc:55-412) on the GPU.
 //
 // Compiled against the reference's UNMODIFIED include/Optimizer.h (signature :48).  The tracking thread calls it after every projection
 // search (Tracking.cc:3222, 3443, 3522).  What stays on the host is the walk over the frame's features under MapPoint::mGlobalMutex
@@ -16,9 +16,9 @@
 namespace ORB_SLAM3 {
 
 int Optimizer::PoseOptimization(Frame* pFrame) {
-    if (pFrame->mpCamera2 || pFrame->Nleft != -1) throw orb_b200::Error("PoseOptimization: a frame with a second camera (Nleft != -1) is not built on the B200 path");
+    if (pFrame->mpCamera2 || pFrame->Nleft != -1) throw orb_b200::Error("PoseOptimization: a frame with a second camera (Nleft != -1) is not built on the GPU path");
     orbx_handle* h = orb_b200_handle_of(pFrame->mpORBextractorLeft);
-    if (!h) throw orb_b200::Error("PoseOptimization: the frame's ORBextractor was not created by the B200 unit");
+    if (!h) throw orb_b200::Error("PoseOptimization: the frame's ORBextractor was not created by the GPU-path unit");
     const int N = pFrame->N;
     std::vector<float> world_pos, obs, inv_sigma2;
     std::vector<int> feature;     // vnIndexEdgeMono / vnIndexEdgeStereo, in one list (feature order)

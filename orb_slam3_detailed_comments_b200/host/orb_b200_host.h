@@ -1,5 +1,5 @@
 // orb_b200_host.h -- shared by the host translation units that stand in for the reference's src/ORBextractor.cc and for the
-// hot members of src/ORBmatcher.cc, src/Frame.cc, src/Optimizer.cc.  They only marshal: all arithmetic runs on the B200 behind
+// hot members of src/ORBmatcher.cc, src/Frame.cc, src/Optimizer.cc.  They only marshal: all arithmetic runs on the GPU behind
 // the C ABI (include/orbslam3_b200.h).  There is no CPU fallback: a failed call throws orb_b200::Error (the reference has no error
 // channel at these call sites; an uncaught exception terminates like its asserts do, a caught one lets the application decide).
 #pragma once
@@ -15,7 +15,7 @@ struct Error : std::runtime_error {
 };
 
 inline void check(orb_status s, const char* what) {
-    if (s != ORB_OK) throw Error(std::string("ORB-SLAM3 B200 path: ") + what + ": " + orb_last_error());
+    if (s != ORB_OK) throw Error(std::string("ORB-SLAM3 GPU path: ") + what + ": " + orb_last_error());
 }
 
 }  // namespace orb_b200

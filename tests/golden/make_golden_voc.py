@@ -15,8 +15,9 @@ sys.path.insert(0, os.path.join(HERE, ".."))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
 import pyref  # noqa: E402
 from orb_slam3_detailed_comments_b200.vocabulary import load_orbvoc_text  # noqa: E402
+from oracle.pyoracle import REFERENCE_ROOT  # noqa: E402
 
-TAR = "/root/reference/Vocabulary/ORBvoc.txt.tar.gz"
+TAR = os.path.join(REFERENCE_ROOT, "Vocabulary", "ORBvoc.txt.tar.gz")
 
 
 def load_full():
@@ -88,7 +89,7 @@ def prune(voc, desc):
                 node_word=voc["node_word"][orig], node_weight=voc["node_weight"][orig], L=voc["L"]), orig
 
 
-FRAME = dict(w=320, h=240, seed=4, sigma=3.0, nrect=20, nfeatures=500)   # a case tests/test_extractor_gpu.py holds bit-exact on a B200
+FRAME = dict(w=320, h=240, seed=4, sigma=3.0, nrect=20, nfeatures=500)   # a case tests/test_extractor_gpu.py holds bit-exact on an H100
 
 
 def frame_descriptors():

@@ -1,4 +1,4 @@
-// tests/host/bow_stub.cc -- TEST INFRASTRUCTURE (CPU tier): orbm_search_bow / orbm_search_bow_keyframes over the oracle instead of the B200,
+// tests/host/bow_stub.cc -- TEST INFRASTRUCTURE (CPU tier): orbm_search_bow / orbm_search_bow_keyframes over the oracle instead of the GPU,
 // so that host/ORBmatcher_bow_b200.cc (FeatureVector merge order, per-feature nodes, written map points) can run without a GPU next to
 // the reference's own functions (oracle/_ref part 2; tests/test_host_bow_vs_ref.py).  The frame "resident on the device" is the one
 // the driver registers with bow_stub_set_frame.  Never linked into the product.

@@ -1,4 +1,4 @@
-// tests/host/fuse_stub.cc -- TEST INFRASTRUCTURE (CPU tier): orbm_search_keyframe over the oracle (orc_search_keyframe) instead of the B200, so that
+// tests/host/fuse_stub.cc -- TEST INFRASTRUCTURE (CPU tier): orbm_search_keyframe over the oracle (orc_search_keyframe) instead of the GPU, so that
 // host/ORBmatcher_fuse_b200.cc (caller-side skips, raw distances through the protected-member access, map mutations in query order) can run
 // without a GPU next to the reference's own function (oracle/_ref part 2; tests/test_host_fuse_vs_ref.py).  Never linked into the product.
 #include <cmath>

@@ -1,4 +1,4 @@
-// tests/host/lba_stub.cc -- TEST INFRASTRUCTURE (CPU tier): lba_solve_bool over the oracle (orc_lba) instead of the B200, so that
+// tests/host/lba_stub.cc -- TEST INFRASTRUCTURE (CPU tier): lba_solve_bool over the oracle (orc_lba) instead of the GPU, so that
 // host/Optimizer_lba_b200.cc -- window selection, flattening, outlier pass, write-back -- can run without a GPU next to the
 // reference's own function (tests/test_host_lba_vs_ref.py).  Never linked into the product.
 #include <cstdint>

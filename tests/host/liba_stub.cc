@@ -1,4 +1,4 @@
-// tests/host/liba_stub.cc -- TEST INFRASTRUCTURE (CPU tier): liba_solve over the oracle (orc_liba) instead of the B200, so that
+// tests/host/liba_stub.cc -- TEST INFRASTRUCTURE (CPU tier): liba_solve over the oracle (orc_liba) instead of the GPU, so that
 // host/Optimizer_liba_b200.cc -- temporal window, fixed keyframes, flattening, outlier pass, failure rule, write-back -- can run without
 // a GPU next to the reference's own function (tests/test_host_liba_vs_ref.py).  liba_link_information (a host-only helper, no device
 // work) comes from liborbslam3_b200.so in both binaries.  Never linked into the product.

@@ -1,5 +1,5 @@
 // tests/host/pose_stub.cc -- TEST INFRASTRUCTURE (CPU tier): orbo_pose_optimization over the oracle (orc_pose_optimization) instead of the
-// B200, so that host/Optimizer_pose_b200.cc -- the feature walk, mvbOutlier, SetPose, the return value -- can run without a GPU next to the
+// GPU, so that host/Optimizer_pose_b200.cc -- the feature walk, mvbOutlier, SetPose, the return value -- can run without a GPU next to the
 // reference's own function (oracle/_ref part 5; tests/test_host_pose_vs_ref.py).  Never linked into the product.
 #include <cstdint>
 #include <vector>

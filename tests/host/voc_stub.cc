@@ -1,5 +1,5 @@
 // tests/host/voc_stub.cc -- TEST INFRASTRUCTURE (CPU tier): orbv_create / orbv_transform over the oracle (orc_bow_transform) instead of the
-// B200, so that host/Frame_bow_b200.cc (vocabulary flattening through the protected-member access, BowVector / FeatureVector filling) can
+// GPU, so that host/Frame_bow_b200.cc (vocabulary flattening through the protected-member access, BowVector / FeatureVector filling) can
 // run without a GPU (tests/test_host_voc_cpu.py).  The frame "resident on the device" is registered by the driver.  Never linked into
 // the product.
 #include <cstdint>

@@ -1,4 +1,4 @@
-"""CPU tier: the C-ABI library builds for sm_100a, loads without a GPU, exports every symbol that
+"""CPU tier: the C-ABI library builds for sm_90a, loads without a GPU, exports every symbol that
 include/orbslam3_b200.h declares, and fails loudly (no CPU fallback) when asked to compute."""
 import ctypes as C
 import os

@@ -19,7 +19,7 @@ MINE = os.path.join(HERE, "host", "fuse_cpu_mine")
 
 
 def _build():
-    if os.path.exists("/root/reference/src/ORBmatcher.cc"):
+    if os.path.exists(os.path.join(po.REFERENCE_ROOT, "src", "ORBmatcher.cc")):
         subprocess.check_call(["bash", os.path.join(HERE, "host", "build_fuse_cpu.sh")])
     return os.path.exists(MINE) and po.build_ref2() is not None
 

@@ -1,7 +1,7 @@
 """CPU tier, build container only: host/Optimizer_lba_b200.cc against the REFERENCE's own Optimizer::LocalBundleAdjustment.
 tests/host/build_lba_cpu.sh cuts the function out of /root/reference/src/Optimizer.cc (and g2o's Levenberg functions out of
 Thirdparty/g2o) and compiles it verbatim over the skeleton map of host/refshim and graph stand-ins whose numerics are the oracle's
-LbaEngine; the host translation unit is linked with lba_solve_bool answered by the oracle (orc_lba) instead of the B200.  Both walk
+LbaEngine; the host translation unit is linked with lba_solve_bool answered by the oracle (orc_lba) instead of the GPU.  Both walk
 the same mock map: window selection (covisible neighbours, bad keyframes, other observers as fixed cameras, the map's initial
 keyframe), vertex / edge construction, the lambda of inertial maps, the stop flag's early exit, optimize(10), the chi2 / depth test
 of every edge (monocular edges first), the erasures on both sides, the pose / point write-back and the counters.  Equality is exact
@@ -12,10 +12,11 @@ import subprocess
 import numpy as np
 import pytest
 
+from oracle.pyoracle import REFERENCE_ROOT
 from orb_slam3_detailed_comments_b200 import synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = REFERENCE_ROOT
 T = os.path.join(ROOT, "tests", "host")
 pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "src", "Optimizer.cc")), reason="reference checkout not present")
 FX, FY, CX, CY, BF, B = 435.2, 435.2, 320.0, 240.0, 47.9, 0.11

@@ -12,6 +12,7 @@ import subprocess
 import numpy as np
 import pytest
 
+from oracle.pyoracle import REFERENCE_ROOT
 from orb_slam3_detailed_comments_b200 import synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -19,12 +20,12 @@ MINE, REF = os.path.join(HERE, "host", "liba_cpu_mine"), os.path.join(HERE, "hos
 
 
 def _build():
-    if os.path.exists("/root/reference/src/Optimizer.cc"):
+    if os.path.exists(os.path.join(REFERENCE_ROOT, "src", "Optimizer.cc")):
         subprocess.check_call(["bash", os.path.join(HERE, "host", "build_liba_cpu.sh")])
     return os.path.exists(MINE) and os.path.exists(REF)
 
 
-pytestmark = pytest.mark.skipif(not _build(), reason="tests/host/liba_cpu_* not built and /root/reference absent")
+pytestmark = pytest.mark.skipif(not _build(), reason="tests/host/liba_cpu_* not built and the reference (ORB_REFERENCE_ROOT) absent")
 
 
 def _quat(R):

@@ -17,7 +17,7 @@ MINE = os.path.join(HERE, "host", "pose_cpu_mine")
 
 
 def _build():
-    if os.path.exists("/root/reference/src/Optimizer.cc"):
+    if os.path.exists(os.path.join(po.REFERENCE_ROOT, "src", "Optimizer.cc")):
         subprocess.check_call(["bash", os.path.join(HERE, "host", "build_pose_cpu.sh")])
     return os.path.exists(MINE) and po.build_ref5() is not None
 

@@ -3,15 +3,17 @@ include/ORBextractor.h, include/ORBmatcher.h, include/Optimizer.h, unchanged -- 
 Frame / KeyFrame / MapPoint / Map come from host/refshim/ref_skeleton.h (their real headers pull in Sophus, g2o, DBoW2, boost and
 Pangolin, none of which exist here); every skeleton member is checked, line by line, against the text of the reference header it
 claims to restate.  Needs /root/reference, so it only runs in the build container; tests/test_zz_host_boundary_gpu.py RUNS the
-same translation units on a B200."""
+same translation units on an H100."""
 import os
 import re
 import subprocess
 
 import pytest
 
+from oracle.pyoracle import REFERENCE_ROOT
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = REFERENCE_ROOT
 HOST = os.path.join(ROOT, "orb_slam3_detailed_comments_b200", "host")
 pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "include", "ORBmatcher.h")), reason="reference checkout not present")
 
@@ -55,7 +57,7 @@ def test_stereo_and_lba_units(tmp_path):
 
 def test_inertial_ba_unit(tmp_path):
     """host/Optimizer_liba_b200.cc against the reference's Optimizer.h; the skeleton's IMU members are behind ORB_REFSHIM_LIBA so that the
-    other units' translation (the binary validated on the B200) does not change."""
+    other units' translation (the binary validated on the GPU) does not change."""
     syms = _compile(tmp_path, "Optimizer_liba_b200", "-DORB_REFSHIM_LIBA")
     assert "T ORB_SLAM3::Optimizer::LocalInertialBA(ORB_SLAM3::KeyFrame*, bool*, ORB_SLAM3::Map*, int&, int&, int&, int&, bool, bool)" in syms
     assert "U liba_solve" in syms and "U liba_link_information" in syms and "g2o" not in syms and "abort" not in syms

@@ -18,7 +18,7 @@ MINE = os.path.join(HERE, "host", "voc_cpu_mine")
 
 
 def _build():
-    if os.path.exists("/root/reference/include/ORBextractor.h"):
+    if os.path.exists(os.path.join(po.REFERENCE_ROOT, "include", "ORBextractor.h")):
         subprocess.check_call(["bash", os.path.join(HERE, "host", "build_voc_cpu.sh")])
     return os.path.exists(MINE)
 

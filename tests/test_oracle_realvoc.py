@@ -15,7 +15,7 @@ from oracle import pyoracle as po
 from orb_slam3_detailed_comments_b200.vocabulary import load_orbvoc_text
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-TAR = "/root/reference/Vocabulary/ORBvoc.txt.tar.gz"
+TAR = os.path.join(po.REFERENCE_ROOT, "Vocabulary", "ORBvoc.txt.tar.gz")
 
 
 @pytest.fixture(scope="module")

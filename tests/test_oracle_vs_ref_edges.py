@@ -68,7 +68,7 @@ def test_pose_only_edges_bitwise(zlo, zhi):
 
 
 def test_device_form_is_the_round_1_oracle():
-    """set_stereo_form(1) is the arithmetic the kernels were validated against on the B200: it reproduces, bit for bit, the vectors the
+    """set_stereo_form(1) is the arithmetic the kernels were validated against on the GPU: it reproduces, bit for bit, the vectors the
     golden file held before the pin (kept under *_devform)."""
     G = np.load(os.path.join(HERE, "golden", "golden_v1.npz"))
     pr = {k[7:]: G[k] for k in G.files if k.startswith("lba_in_")}

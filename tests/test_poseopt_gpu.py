@@ -49,12 +49,21 @@ def ex():
     e.close()
 
 
-def _check(g, f):
+def _check(g, f, ulp_spread=False):
     r = po.pose_optimization(f["pose"], f["world_pos"], f["obs"], f["inv_sigma2"], np.float32(CAM5))
     # near convergence the gain ratio is rounding noise, so an accept / reject may flip without moving the pose: the rounds
-    # must agree, the LM iteration / trial counts within a couple of steps
-    assert g["rounds"] == r["rounds"] and abs(g["iterations"] - r["iterations"]) <= 2 and abs(g["trials"] - r["trials"]) <= 4, \
-        (g["rounds"], g["iterations"], g["trials"], r["rounds"], r["iterations"], r["trials"])
+    # must agree, the LM iteration / trial counts within a couple of steps of the oracle -- or, with ulp_spread, of the range
+    # the oracle's own counts span when the map points move by one ulp (frames whose counts rounding noise decides)
+    its, trials = [r["iterations"]], [r["trials"]]
+    if ulp_spread:
+        for k in range(8):
+            step = np.random.default_rng(k).choice([-1, 0, 1], f["world_pos"].shape) * np.float32(2 ** -23)
+            rk = po.pose_optimization(f["pose"], (f["world_pos"] * (1 + step)).astype(np.float32), f["obs"], f["inv_sigma2"], np.float32(CAM5))
+            assert rk["rounds"] == r["rounds"] and np.abs(rk["pose"] - r["pose"]).max() < TOL
+            its.append(rk["iterations"])
+            trials.append(rk["trials"])
+    assert g["rounds"] == r["rounds"] and min(its) - 2 <= g["iterations"] <= max(its) + 2 and min(trials) - 4 <= g["trials"] <= max(trials) + 4, \
+        (g["rounds"], g["iterations"], g["trials"], r["rounds"], its, trials)
     assert np.abs(g["pose"] - r["pose"]).max() < TOL
     assert abs(g["inliers"] - r["inliers"]) <= 1 and int((g["outlier"] != r["outlier"]).sum()) <= 1   # a chi2 within 1e-9 of the threshold
     return r
@@ -85,11 +94,12 @@ def test_degenerate_frames(ex):
 
 def test_all_outliers_after_first_round(ex):
     """Every observation is garbage: after round 0 nothing is active, the later rounds only re-classify (the reference's
-    optimize() returns without touching the vertex)."""
+    optimize() returns without touching the vertex).  Fitting garbage, LM stops where rounding noise says: one-ulp changes of the
+    map points move the oracle's own iteration count from 23 to 29 at the same pose, so the counts are held to that spread."""
     f = make_frame(20, 200, outlier_frac=1.0)
     f["obs"][:, :2] += 200
     g = PoseOptimization(ex, [f], CAM5)[0]
-    _check(g, f)
+    _check(g, f, ulp_spread=True)
 
 
 def test_edges_from_device_matches_and_optimise():

@@ -171,7 +171,7 @@ def run_mt(exe, c, W, H, N, variant, threads, tmp_path):
 @pytest.mark.parametrize("variant,threads", [(0, 3), (0, 8), (1, 3), (1, 8), (1, 32), (1, 64)])     # variant 1 also runs 1024-thread CTAs
 def test_threaded_quadtree_is_race_free_and_matches_oracle(qt_mt, tmp_path, variant, threads):
     """Real FAST candidates of a 640x480 frame, all 8 levels: T threads + a real barrier + ThreadSanitizer.  Variant 0 is the kernel
-    that ran green on a B200 in round 1 (so this also says the harness agrees with the device about where barriers are needed);
+    that ran green on the GPU tier (so this also says the harness agrees with the device about where barriers are needed);
     variant 1 is the CTA-parallel ordered-phase sort."""
     ex = po.OracleExtractor(1200, 1.2, 8, 20, 7)
     ex(synth.frame(640, 480, 1))

@@ -1,6 +1,6 @@
-"""CPU tier: the machine code the library ships is the machine code whose `pytest -m gpu` run was green on a B200.
-profiles/r02_sass_fingerprints.json is taken (scripts/sass_fingerprint.py) from the build that last passed the whole GPU tier
-(every kernel has had a device run since round 2: UNPROVEN is empty).  An intentional kernel change must come with a GPU run and a
+"""CPU tier: the machine code the library ships is the machine code whose `pytest -m gpu` run was green on an H100.
+tests/golden/sass_fingerprints.json is taken (scripts/sass_fingerprint.py) from the sm_90a build that last passed the whole GPU tier
+(every kernel has had a device run: UNPROVEN is empty).  An intentional kernel change must come with a GPU run and a
 refreshed fingerprint file; an unintentional one (a shared header edit that changes another kernel's code) fails here first."""
 import importlib.util
 import json
@@ -21,7 +21,7 @@ def test_validated_kernels_are_bit_identical():
     from orb_slam3_detailed_comments_b200 import _native as N
     N.build()
     now = mod.fingerprints()
-    ref = json.load(open(os.path.join(ROOT, "profiles", "r02_sass_fingerprints.json")))
+    ref = json.load(open(os.path.join(ROOT, "tests", "golden", "sass_fingerprints.json")))
     proven = {k: v for k, v in ref.items() if not any(u in k for u in UNPROVEN)}
     assert len(proven) >= 24
     for k, v in proven.items():

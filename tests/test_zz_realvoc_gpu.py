@@ -1,7 +1,7 @@
 """GPU tier (runs last): orbv_transform over a pruned copy of the REAL ORBvoc.txt tree (tests/golden/orbvoc_subtree.npz: real node
 descriptors and idf weights, 2..10 children per node, leaves at several depths, zero-weight words, childless pruned branches)
 against the CPU oracle, on the descriptors the extractor produced.  Added after round 1's last GPU run, so it sorts after the
-suites that have been green on a B200; the kernel path is the one tests/test_bow_gpu.py covers on synthetic uniform trees."""
+suites that have been green on an H100; the kernel path is the one tests/test_bow_gpu.py covers on synthetic uniform trees."""
 import os
 
 import numpy as np

@@ -1,5 +1,5 @@
-// Issue rate of the integer instructions the extractor kernels are made of (IMAD, IDP, VABSDIFF4, IADD3, LOP3, PRMT, SHF, VIMNMX3, POPC) on sm_100a: 8 independent chains per thread, 1024 threads per CTA, one CTA per SM.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o idp_rate idp_rate.cu && ./idp_rate
+// Issue rate of the integer instructions the extractor kernels are made of (IMAD, IDP, VABSDIFF4, IADD3, LOP3, PRMT, SHF, VIMNMX3, POPC) on sm_90a: 8 independent chains per thread, 1024 threads per CTA, one CTA per SM.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o idp_rate idp_rate.cu && ./idp_rate
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
