@@ -170,36 +170,29 @@ extern "C" orb_status orbv_transform(orbx_handle* h, const orbv_vocabulary* voc,
     if (!h || !voc || !word_out || !node_out || !weight_out) return set_error(ORB_ERR_INVALID, "bad arguments");
     if (voc->device != h->cfg.device) return set_error(ORB_ERR_INVALID, "vocabulary and extractor live on different devices");
     ORB_CUDA(cudaSetDevice(h->cfg.device));
-    orb_status s = orbx_counts(h, nullptr, nullptr, nullptr);
+    int rows = 0;
+    orb_status s = batch_rows(h, &rows);
     if (s != ORB_OK) return s;
-    const int nimg = h->last_batch, MB = h->cfg.max_batch;
-    const int rows = h->h_counts[2 * MB + nimg];
+    const int nimg = h->last_batch;
     const bool dev = on_device != 0, want_bow = bow_count_out && bow_word_out && bow_weight_out;
     const int maxFeat = h->geom.kpTotal;
-    const size_t need = dev ? 4096 : (size_t)std::max(rows, 1) * 16 + (want_bow ? (size_t)nimg * (4 + (size_t)maxFeat * 12) : 0) + 65536;
-    if (need > h->po_bytes) {     // results staging shares the pose-optimisation buffer (not the matcher stage: its feature_node input may live there)
-        if (h->d_po) cudaFree(h->d_po);
-        h->d_po = nullptr;
-        h->po_bytes = 0;
-        const size_t want = (need + (1 << 20)) / (1 << 20) * (1 << 20);
-        ORB_CUDA(cudaMalloc((void**)&h->d_po, want));
-        h->po_bytes = want;
-    }
-    size_t off = 0;
-    auto take = [&](size_t bytes) { off = (off + 255) / 256 * 256; uint8_t* p = h->d_po + off; off += bytes; return p; };
     BowParams P{};
     P.child_off = voc->d_child_off; P.child = voc->d_child; P.ndesc = voc->d_desc; P.nword = voc->d_word; P.nweight = voc->d_weight;
     P.nid_level = voc->L - levelsup;
     P.desc = h->d_desc; P.rows = rows;
-    P.word = dev ? word_out : reinterpret_cast<int*>(take((size_t)std::max(rows, 1) * 4));
-    P.node = dev ? node_out : reinterpret_cast<int*>(take((size_t)std::max(rows, 1) * 4));
-    P.weight = dev ? weight_out : reinterpret_cast<double*>(take((size_t)std::max(rows, 1) * 8));
     P.offsets = h->d_offsets; P.nkp = h->d_nkp; P.maxFeat = maxFeat;
-    if (want_bow) {
-        P.bow_count = dev ? bow_count_out : reinterpret_cast<int*>(take((size_t)nimg * 4));
-        P.bow_word = dev ? bow_word_out : reinterpret_cast<int*>(take((size_t)nimg * maxFeat * 4));
-        P.bow_weight = dev ? bow_weight_out : reinterpret_cast<double*>(take((size_t)nimg * maxFeat * 8));
-    }
+    // results staging shares the pose-optimisation buffer (not the matcher stage: its feature_node input may live there)
+    auto layout = [&](Carve& c) {
+        P.word = dev ? word_out : c.take<int>(rows);
+        P.node = dev ? node_out : c.take<int>(rows);
+        P.weight = dev ? weight_out : c.take<double>(rows);
+        if (want_bow) {
+            P.bow_count = dev ? bow_count_out : c.take<int>(nimg);
+            P.bow_word = dev ? bow_word_out : c.take<int>((size_t)nimg * maxFeat);
+            P.bow_weight = dev ? bow_weight_out : c.take<double>((size_t)nimg * maxFeat);
+        }
+    };
+    if ((s = carve_scratch(h->po_bytes, h->d_po, h->capturing, h->stream, layout)) != ORB_OK) return s;
     cudaStream_t st = h->stream;
     if (rows > 0) {
         k_bow_transform<<<(rows * 16 + 255) / 256, 256, 0, st>>>(P);

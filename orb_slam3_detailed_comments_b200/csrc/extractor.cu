@@ -620,10 +620,16 @@ extern "C" orb_status orbx_counts(orbx_handle* h, int32_t* n, int32_t* mono_inde
     return ORB_OK;
 }
 
+orb_status batch_rows(orbx_handle* h, int* rows) {
+    const orb_status s = orbx_counts(h, nullptr, nullptr, nullptr);
+    if (s == ORB_OK) *rows = h->h_counts[2 * h->cfg.max_batch + h->last_batch];
+    return s;
+}
+
 extern "C" orb_status orbx_download(orbx_handle* h, orbx_keypoint* kps, uint8_t* desc, int32_t cap_rows) {
-    orb_status s = orbx_counts(h, nullptr, nullptr, nullptr);
+    int total = 0;
+    orb_status s = batch_rows(h, &total);
     if (s != ORB_OK) return s;
-    const int total = h->h_counts[2 * h->cfg.max_batch + h->last_batch];
     const int rows = std::min(total, (int)cap_rows);
     if (rows > 0) {
         if (kps) ORB_CUDA(cudaMemcpyAsync(kps, h->d_kps, sizeof(orbx_keypoint) * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));

@@ -3,9 +3,11 @@
 #include <vector>
 
 #include "common.cuh"
+#include "scratch.h"
 
 struct orbr_state;
 void orbr_release(struct orbx_handle* h);   // replay.cu
+orb_status batch_rows(struct orbx_handle* h, int* rows);   // extractor.cu: compact rows of the last batch (orbx_counts)
 
 struct orbx_handle {
     orbx_config cfg{};

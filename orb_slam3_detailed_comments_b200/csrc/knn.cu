@@ -159,17 +159,6 @@ __global__ void __launch_bounds__(KNN_THREADS) k_hamming_knn2(const __grid_const
     }
 }
 
-orb_status knn_stage(orbx_handle* h, size_t need) {
-    if (need <= h->po_bytes) return ORB_OK;
-    if (h->d_po) cudaFree(h->d_po);
-    h->d_po = nullptr;
-    h->po_bytes = 0;
-    const size_t want = need + need / 4 + (1 << 20);
-    ORB_CUDA(cudaMalloc((void**)&h->d_po, want));
-    h->po_bytes = want;
-    return ORB_OK;
-}
-
 }  // namespace
 
 extern "C" orb_status orbm_hamming_knn2(orbx_handle* h, int32_t n_pairs, const int32_t* query_offset, const uint8_t* query_desc,
@@ -188,24 +177,18 @@ extern "C" orb_status orbm_hamming_knn2(orbx_handle* h, int32_t n_pairs, const i
     if (nq == 0) return ORB_OK;
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     const size_t np = (size_t)n_pairs;
-    orb_status s = knn_stage(h, 2 * (np + 1) * 4 + ((size_t)nq + (size_t)nt) * 32 + (size_t)nq * 16 + 8 * 256);
-    if (s != ORB_OK) return s;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { off = (off + 255) / 256 * 256; uint8_t* p = h->d_po + off; off += bytes; return p; };
     KnnParams P;
     P.n_pairs = n_pairs;
-    int* d_qo = reinterpret_cast<int*>(take((np + 1) * 4));
-    int* d_to = reinterpret_cast<int*>(take((np + 1) * 4));
-    uint8_t* d_q = take((size_t)nq * 32);
-    uint8_t* d_t = take((size_t)std::max(nt, 1) * 32);
-    P.idx = reinterpret_cast<int*>(take((size_t)nq * 8));
-    P.dist = reinterpret_cast<int*>(take((size_t)nq * 8));
-    P.q_off = d_qo; P.t_off = d_to; P.q_desc = d_q; P.t_desc = d_t;
     cudaStream_t st = h->stream;
-    ORB_CUDA(cudaMemcpyAsync(d_qo, query_offset, (np + 1) * 4, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_to, train_offset, (np + 1) * 4, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_q, query_desc, (size_t)nq * 32, cudaMemcpyHostToDevice, st));
-    if (nt) ORB_CUDA(cudaMemcpyAsync(d_t, train_desc, (size_t)nt * 32, cudaMemcpyHostToDevice, st));
+    auto layout = [&](Carve& c) {
+        P.q_off = stage_in(c, query_offset, np + 1, false); P.t_off = stage_in(c, train_offset, np + 1, false);
+        P.q_desc = stage_in(c, query_desc, (size_t)nq * 32, false);
+        P.t_desc = train_desc ? stage_in(c, train_desc, (size_t)nt * 32, false) : c.take<uint8_t>(32);   // a real address even with no train rows
+        P.idx = c.take<int>((size_t)nq * 2);
+        P.dist = c.take<int>((size_t)nq * 2);
+    };
+    const orb_status s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
+    if (s != ORB_OK) return s;
     const char* tma = getenv("ORB_KNN_TMA");       // 1: train tiles by cp.async.bulk + mbarrier, double-buffered
     if (tma && atoi(tma) == 1) k_hamming_knn2_tma<<<dim3((maxq + KNN_THREADS - 1) / KNN_THREADS, n_pairs), KNN_THREADS, 0, st>>>(P);
     else k_hamming_knn2<<<dim3((maxq + KNN_THREADS - 1) / KNN_THREADS, n_pairs), KNN_THREADS, 0, st>>>(P);

@@ -9,6 +9,7 @@
 
 #include "common.cuh"
 #include "liba_pack.h"
+#include "scratch.h"
 
 using namespace orb;
 
@@ -100,18 +101,8 @@ extern "C" orb_status liba_solve(liba_handle* h, int32_t n_problems, const liba_
         base[i] = total;
         total += (lay[i].total + 255) & ~(size_t)255;
     }
-    if (total > h->d_bytes) {
-        if (h->d_buf) cudaFree(h->d_buf);
-        h->d_buf = nullptr; h->d_bytes = 0;
-        ORB_CUDA(cudaMalloc((void**)&h->d_buf, total + total / 4));
-        h->d_bytes = total + total / 4;
-    }
-    if (total > h->h_bytes) {
-        if (h->h_buf) cudaFreeHost(h->h_buf);
-        h->h_buf = nullptr; h->h_bytes = 0;
-        ORB_CUDA(cudaMallocHost((void**)&h->h_buf, total + total / 4));
-        h->h_bytes = total + total / 4;
-    }
+    orb_status s = grow_device(h->d_bytes, h->d_buf, total, false);
+    if (s != ORB_OK || (s = grow_pinned(h->h_bytes, h->h_buf, total)) != ORB_OK) return s;
     LibaDev* hdev = reinterpret_cast<LibaDev*>(h->h_buf);
     ORB_CUDA(cudaMemsetAsync(h->d_buf, 0, total, h->stream));
     for (int i = 0; i < n_problems; ++i) liba_pack(in[i], h->h_buf + base[i], h->d_buf + base[i], &hdev[i]);

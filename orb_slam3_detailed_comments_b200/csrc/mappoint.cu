@@ -77,17 +77,6 @@ __global__ void __launch_bounds__(128) k_normal_depth(int np, const int* __restr
 
 }  // namespace orb
 
-static orb_status po_stage(orbx_handle* h, size_t need) {
-    if (need <= h->po_bytes) return ORB_OK;
-    if (h->d_po) cudaFree(h->d_po);
-    h->d_po = nullptr;
-    h->po_bytes = 0;
-    const size_t want = (need + (1 << 20)) / (1 << 20) * (1 << 20);
-    ORB_CUDA(cudaMalloc((void**)&h->d_po, want));
-    h->po_bytes = want;
-    return ORB_OK;
-}
-
 extern "C" orb_status orbp_distinctive_descriptors(orbx_handle* h, int32_t n_points, const int32_t* obs_offset, const uint8_t* obs_desc,
                                                    int32_t* best_index_out) {
     if (!h || n_points < 0 || !obs_offset || !best_index_out) return set_error(ORB_ERR_INVALID, "bad arguments");
@@ -97,14 +86,15 @@ extern "C" orb_status orbp_distinctive_descriptors(orbx_handle* h, int32_t n_poi
     for (int i = 0; i < n_points; ++i)
         if (obs_offset[i + 1] - obs_offset[i] > 65535) return set_error(ORB_ERR_UNSUPPORTED, "map point with more than 65535 observations");
     ORB_CUDA(cudaSetDevice(h->cfg.device));
-    orb_status s = po_stage(h, (size_t)n_points * 8 + (size_t)nobs * 32 + 4096);
-    if (s != ORB_OK) return s;
-    int* d_off = reinterpret_cast<int*>(h->d_po);
-    int* d_best = d_off + (((size_t)n_points + 1 + 63) / 64) * 64;
-    uint8_t* d_desc = reinterpret_cast<uint8_t*>(d_best + (((size_t)n_points + 63) / 64) * 64);
     cudaStream_t st = h->stream;
-    ORB_CUDA(cudaMemcpyAsync(d_off, obs_offset, sizeof(int) * ((size_t)n_points + 1), cudaMemcpyHostToDevice, st));
-    if (nobs) ORB_CUDA(cudaMemcpyAsync(d_desc, obs_desc, (size_t)nobs * 32, cudaMemcpyHostToDevice, st));
+    const int* d_off; const uint8_t* d_desc; int* d_best;
+    auto layout = [&](Carve& c) {
+        d_off = stage_in(c, obs_offset, (size_t)n_points + 1, false);
+        d_best = c.take<int>(n_points);
+        d_desc = stage_in(c, obs_desc, (size_t)nobs * 32, false);
+    };
+    const orb_status s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
+    if (s != ORB_OK) return s;
     k_distinctive<<<n_points, 32, 0, st>>>(d_off, d_desc, d_best);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
@@ -125,30 +115,17 @@ extern "C" orb_status orbp_update_normal_and_depth(orbx_handle* h, int32_t n_poi
         if (ref_level[i] < 0 || ref_level[i] >= h->cfg.n_levels) return set_error(ORB_ERR_INVALID, "reference level outside the pyramid");
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     const size_t np = (size_t)n_points;
-    orb_status s = po_stage(h, np * (4 + 12 + 12 + 4 + 12 + 4 + 4) + (size_t)nobs * 12 + 64 * 4 + 8192);
-    if (s != ORB_OK) return s;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { off = (off + 255) / 256 * 256; uint8_t* p = h->d_po + off; off += bytes; return p; };
-    int* d_off = reinterpret_cast<int*>(take((np + 1) * 4));
-    float* d_oc = reinterpret_cast<float*>(take((size_t)std::max(nobs, 1) * 12));
-    float* d_pos = reinterpret_cast<float*>(take(np * 12));
-    float* d_rc = reinterpret_cast<float*>(take(np * 12));
-    int* d_lv = reinterpret_cast<int*>(take(np * 4));
-    float* d_sc = reinterpret_cast<float*>(take(64 * 4));
-    float* d_n = reinterpret_cast<float*>(take(np * 12));
-    float* d_mx = reinterpret_cast<float*>(take(np * 4));
-    float* d_mn = reinterpret_cast<float*>(take(np * 4));
     cudaStream_t st = h->stream;
-    ORB_CUDA(cudaMemcpyAsync(d_off, obs_offset, (np + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (nobs) ORB_CUDA(cudaMemcpyAsync(d_oc, obs_center, (size_t)nobs * 12, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_pos, world_pos, np * 12, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_rc, ref_center, np * 12, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_lv, ref_level, np * 4, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_sc, h->scale.data(), sizeof(float) * (size_t)h->cfg.n_levels, cudaMemcpyHostToDevice, st));
-    // outputs start from the caller's current values: points without observations keep them
-    ORB_CUDA(cudaMemcpyAsync(d_n, normal_out, np * 12, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_mx, max_dist_out, np * 4, cudaMemcpyHostToDevice, st));
-    ORB_CUDA(cudaMemcpyAsync(d_mn, min_dist_out, np * 4, cudaMemcpyHostToDevice, st));
+    const int *d_off, *d_lv; const float *d_oc, *d_pos, *d_rc, *d_sc; float *d_n, *d_mx, *d_mn;
+    auto layout = [&](Carve& c) {
+        d_off = stage_in(c, obs_offset, np + 1, false); d_oc = stage_in(c, obs_center, (size_t)nobs * 3, false);
+        d_pos = stage_in(c, world_pos, np * 3, false); d_rc = stage_in(c, ref_center, np * 3, false);
+        d_lv = stage_in(c, ref_level, np, false); d_sc = stage_in(c, h->scale.data(), (size_t)h->cfg.n_levels, false);
+        // outputs start from the caller's current values: points without observations keep them
+        d_n = stage_in(c, normal_out, np * 3, false); d_mx = stage_in(c, max_dist_out, np, false); d_mn = stage_in(c, min_dist_out, np, false);
+    };
+    const orb_status s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
+    if (s != ORB_OK) return s;
     k_normal_depth<<<(n_points + 127) / 128, 128, 0, st>>>(n_points, d_off, d_oc, d_pos, d_rc, d_lv, d_sc, h->cfg.n_levels, d_n, d_mx, d_mn);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());

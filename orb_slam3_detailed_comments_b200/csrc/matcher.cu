@@ -1173,30 +1173,6 @@ __global__ void __launch_bounds__(256) k_in_frustum(const __grid_constant__ Frus
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static orb_status ensure_stage(orbx_handle* h, size_t bytes) {
-    if (bytes <= h->stage_bytes) return ORB_OK;
-    if (h->capturing) return set_error(ORB_ERR_INVALID, "scratch must be sized by one eager call with the same bounds before a graph capture");
-    if (h->d_stage) cudaFree(h->d_stage);
-    h->d_stage = nullptr;
-    h->stage_bytes = 0;
-    const size_t want = (bytes + (1 << 20)) / (1 << 20) * (1 << 20);
-    ORB_CUDA(cudaMalloc((void**)&h->d_stage, want));
-    h->stage_bytes = want;
-    return ORB_OK;
-}
-
-struct StageCursor {
-    uint8_t* base;
-    size_t off = 0;
-    template <typename T>
-    T* take(size_t n) {
-        off = (off + 255) / 256 * 256;
-        T* p = reinterpret_cast<T*>(base + off);
-        off += n * sizeof(T);
-        return p;
-    }
-};
-
 static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int max_q_per_frame) {
     cudaStream_t st = h->stream;
     const size_t fsm = ((size_t)P.maxFeat * 23 + 16 + 15) / 16 * 16;
@@ -1258,12 +1234,29 @@ static void fill_frame_side(orbx_handle* h, const orbm_camera* cam, ProjParams& 
     for (int l = 0; l < ORB_MAX_LEVELS; ++l) P.scale[l] = l < h->cfg.n_levels ? h->scale[l] : 1.f;
 }
 
-template <typename T>
-static orb_status upload(orbx_handle* h, T*& dst, const T* src, size_t n, StageCursor& cur, bool on_device) {
-    if (!src) { dst = nullptr; return ORB_OK; }
-    if (on_device) { dst = const_cast<T*>(src); return ORB_OK; }
-    dst = cur.take<T>(n);
-    ORB_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
+// Query counts of a per-frame search (total, largest frame) and the rows of the batch.  Host tables are read in place, device
+// tables are read back; bounded (orbm_set_device_query_bounds), the bounds stand in and nothing is read back.
+static orb_status frame_table(orbx_handle* h, int nf, const int32_t* frame_image, const int32_t* query_offset, bool dev, bool bounded,
+                              int& nq, int& maxq, int& rows) {
+    rows = h->rows_bound > 0 ? h->rows_bound : (int)h->out_rows;
+    orb_status s;
+    if (!bounded && (s = batch_rows(h, &rows)) != ORB_OK) return s;
+    std::vector<int> qoff_h(nf + 1, 0), fimg_h(nf, 0);
+    if (dev && !bounded) {
+        ORB_CUDA(cudaMemcpyAsync(qoff_h.data(), query_offset, sizeof(int) * (nf + 1), cudaMemcpyDeviceToHost, h->stream));
+        ORB_CUDA(cudaMemcpyAsync(fimg_h.data(), frame_image, sizeof(int) * nf, cudaMemcpyDeviceToHost, h->stream));
+        ORB_CUDA(cudaStreamSynchronize(h->stream));
+    } else if (!dev) {
+        std::copy(query_offset, query_offset + nf + 1, qoff_h.begin());
+        std::copy(frame_image, frame_image + nf, fimg_h.begin());
+    }
+    nq = qoff_h[nf];
+    maxq = 0;
+    for (int f = 0; f < nf; ++f) {
+        maxq = std::max(maxq, qoff_h[f + 1] - qoff_h[f]);
+        if (fimg_h[f] < 0 || fimg_h[f] >= h->last_batch || qoff_h[f + 1] < qoff_h[f]) return set_error(ORB_ERR_INVALID, "bad frame table");
+    }
+    if (bounded) { nq = h->q_total_bound; maxq = h->q_frame_bound; }   // upper bounds: the kernels take the real counts from the device tables
     return ORB_OK;
 }
 
@@ -1282,64 +1275,29 @@ extern "C" orb_status orbm_search_local_points(orbx_handle* h, const orbm_camera
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     const bool dev = Q->on_device != 0;
     const bool bounded = dev && h->q_total_bound > 0;   // orbm_set_device_query_bounds: nothing is read back, no synchronisation
-    orb_status s = ORB_OK;
-    size_t rows = (size_t)(h->rows_bound > 0 ? h->rows_bound : (int)h->out_rows);
-    if (!bounded) {
-        s = orbx_counts(h, nullptr, nullptr, nullptr);   // total compact rows of the batch
-        if (s != ORB_OK) return s;
-        rows = (size_t)h->h_counts[2 * h->cfg.max_batch + h->last_batch];
-    }
     const int nf = Q->n_frames;
-    std::vector<int> qoff_h(nf + 1), fimg_h(nf);
-    if (bounded) {
-        for (int f = 0; f <= nf; ++f) qoff_h[f] = 0;
-        for (int f = 0; f < nf; ++f) fimg_h[f] = 0;
-    } else if (dev) {
-        ORB_CUDA(cudaMemcpyAsync(qoff_h.data(), Q->query_offset, sizeof(int) * (nf + 1), cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaMemcpyAsync(fimg_h.data(), Q->frame_image, sizeof(int) * nf, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-    } else {
-        std::copy(Q->query_offset, Q->query_offset + nf + 1, qoff_h.begin());
-        std::copy(Q->frame_image, Q->frame_image + nf, fimg_h.begin());
-    }
-    int nq = qoff_h[nf];
-    int maxq = 0;
-    for (int f = 0; f < nf; ++f) {
-        maxq = std::max(maxq, qoff_h[f + 1] - qoff_h[f]);
-        if (fimg_h[f] < 0 || fimg_h[f] >= h->last_batch || qoff_h[f + 1] < qoff_h[f]) return set_error(ORB_ERR_INVALID, "bad frame table");
-    }
-    if (bounded) { nq = h->q_total_bound; maxq = h->q_frame_bound; }   // upper bounds: the kernels take the real counts from the device tables
-    const size_t need = (size_t)nq * (PM_K * 8 + 4 + 4 * 6 + 32 + 8) + rows + (size_t)nf * (16 + 2 * (size_t)h->geom.kpTotal + 2 * 3073 + 512) + 65536;
-    if ((s = ensure_stage(h, need)) != ORB_OK) return s;
-    StageCursor cur{h->d_stage};
+    int nq, maxq, rows;
+    orb_status s = frame_table(h, nf, Q->frame_image, Q->query_offset, dev, bounded, nq, maxq, rows);
+    if (s != ORB_OK) return s;
     ProjParams P{};
     fill_frame_side(h, cam, P);
     P.mode = 0;
-    int* d_fimg; int* d_qoff;
-    if ((s = upload(h, d_fimg, (const int*)Q->frame_image, nf, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, d_qoff, (const int*)Q->query_offset, nf + 1, cur, dev)) != ORB_OK) return s;
-    P.frame_image = d_fimg; P.qoff = d_qoff;
-    float *a0, *a1, *a2, *f0, *f1; int* lvl; uint8_t *qd, *fl;
-    if ((s = upload(h, a0, Q->proj_x, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, a1, Q->proj_y, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, a2, Q->proj_xr, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, lvl, (const int*)Q->level, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, f0, Q->view_cos, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, f1, Q->track_depth, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, qd, Q->desc, (size_t)nq * 32, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, fl, Q->feature_claimed, rows, cur, dev)) != ORB_OK) return s;
-    uint8_t* qv;
-    if ((s = upload(h, qv, Q->in_view, nq, cur, dev)) != ORB_OK) return s;
-    P.qvalid = qv;
-    P.a0 = a0; P.a1 = a1; P.a2 = a2; P.level = lvl; P.f0 = f0; P.f1 = f1; P.qdesc = qd; P.flag = fl;
     P.th = th; P.nnratio = nnratio; P.bFar = far_points; P.thFar = th_far;
-    P.gridOrder = cur.take<uint16_t>((size_t)nf * P.maxFeat);
-    P.gridStart = cur.take<uint16_t>((size_t)nf * (GRID_COLS * GRID_ROWS + 1));
-    P.topk = cur.take<unsigned long long>((size_t)nq * PM_K);
-    P.cnt = cur.take<int>(nq);
-    P.match = dev ? match_out : cur.take<int>(nq);
-    P.nmatches = (dev && nmatches_out) ? nmatches_out : cur.take<int>(nf);
-    P.seqFlag = cur.take<int>(nf);
+    auto layout = [&](Carve& c) {
+        P.frame_image = stage_in(c, Q->frame_image, nf, dev); P.qoff = stage_in(c, Q->query_offset, nf + 1, dev);
+        P.a0 = stage_in(c, Q->proj_x, nq, dev); P.a1 = stage_in(c, Q->proj_y, nq, dev); P.a2 = stage_in(c, Q->proj_xr, nq, dev);
+        P.level = stage_in(c, Q->level, nq, dev); P.f0 = stage_in(c, Q->view_cos, nq, dev); P.f1 = stage_in(c, Q->track_depth, nq, dev);
+        P.qdesc = stage_in(c, Q->desc, (size_t)nq * 32, dev); P.flag = stage_in(c, Q->feature_claimed, rows, dev);
+        P.qvalid = stage_in(c, Q->in_view, nq, dev);
+        P.gridOrder = c.take<uint16_t>((size_t)nf * P.maxFeat);
+        P.gridStart = c.take<uint16_t>((size_t)nf * (GRID_COLS * GRID_ROWS + 1));
+        P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
+        P.cnt = c.take<int>(nq);
+        P.match = dev ? match_out : c.take<int>(nq);
+        P.nmatches = (dev && nmatches_out) ? nmatches_out : c.take<int>(nf);
+        P.seqFlag = c.take<int>(nf);
+    };
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     ORB_CUDA(cudaMemsetAsync(P.seqFlag, 0, sizeof(int) * nf, h->stream));
     if (nq > 0 && (s = launch_proj(h, P, nf, maxq)) != ORB_OK) return s;
     if (dev && nq == 0 && nmatches_out) ORB_CUDA(cudaMemsetAsync(nmatches_out, 0, sizeof(int) * nf, h->stream));   // no kernel ran: a consumer must not see the previous step's counts
@@ -1360,61 +1318,31 @@ extern "C" orb_status orbm_search_last_frame(orbx_handle* h, const orbm_camera* 
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     const bool dev = Q->on_device != 0;
     const bool bounded = dev && h->q_total_bound > 0;   // orbm_set_device_query_bounds: nothing is read back, no synchronisation
-    orb_status s = ORB_OK;
-    int total_rows = h->rows_bound > 0 ? h->rows_bound : (int)h->out_rows;
-    if (!bounded) {
-        s = orbx_counts(h, nullptr, nullptr, nullptr);   // total compact rows of the batch
-        if (s != ORB_OK) return s;
-        total_rows = h->h_counts[2 * h->cfg.max_batch + h->last_batch];
-    }
     const int nf = Q->n_frames;
-    std::vector<int> qoff_h(nf + 1), fimg_h(nf);
-    if (bounded) {
-        for (int f = 0; f <= nf; ++f) qoff_h[f] = 0;
-        for (int f = 0; f < nf; ++f) fimg_h[f] = 0;
-    } else if (dev) {
-        ORB_CUDA(cudaMemcpyAsync(qoff_h.data(), Q->query_offset, sizeof(int) * (nf + 1), cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaMemcpyAsync(fimg_h.data(), Q->frame_image, sizeof(int) * nf, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-    } else {
-        std::copy(Q->query_offset, Q->query_offset + nf + 1, qoff_h.begin());
-        std::copy(Q->frame_image, Q->frame_image + nf, fimg_h.begin());
-    }
-    int nq = qoff_h[nf];
-    int maxq = 0;
-    for (int f = 0; f < nf; ++f) {
-        maxq = std::max(maxq, qoff_h[f + 1] - qoff_h[f]);
-        if (fimg_h[f] < 0 || fimg_h[f] >= h->last_batch || qoff_h[f + 1] < qoff_h[f]) return set_error(ORB_ERR_INVALID, "bad frame table");
-    }
-    if (bounded) { nq = h->q_total_bound; maxq = h->q_frame_bound; }
-    const size_t need = (size_t)nq * (PM_K * 8 + 4 + 4 + 12 + 4 + 4 + 32 + 1 + 16) + (size_t)total_rows * 4 + (size_t)nf * (64 + 2 * (size_t)h->geom.kpTotal + 2 * 3073 + 512) + 65536;
-    if ((s = ensure_stage(h, need)) != ORB_OK) return s;
-    StageCursor cur{h->d_stage};
+    int nq, maxq, total_rows;
+    orb_status s = frame_table(h, nf, Q->frame_image, Q->query_offset, dev, bounded, nq, maxq, total_rows);
+    if (s != ORB_OK) return s;
     ProjParams P{};
     fill_frame_side(h, cam, P);
     P.mode = 1;
-    int *d_fimg, *d_qoff, *d_dir, *lvl; float *xw, *ang, *tcw; uint8_t *qd, *ob;
-    if ((s = upload(h, d_fimg, (const int*)Q->frame_image, nf, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, d_qoff, (const int*)Q->query_offset, nf + 1, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, tcw, Q->Tcw, (size_t)nf * 7, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, d_dir, (const int*)Q->direction, nf, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, xw, Q->world_pos, (size_t)nq * 3, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, lvl, (const int*)Q->last_octave, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, ang, Q->last_angle, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, qd, Q->desc, (size_t)nq * 32, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, ob, Q->obs_positive, nq, cur, dev)) != ORB_OK) return s;
-    P.frame_image = d_fimg; P.qoff = d_qoff; P.Tcw = tcw; P.direction = d_dir;
-    P.a0 = xw; P.level = lvl; P.f0 = ang; P.qdesc = qd; P.flag = ob;
     P.th = th; P.checkOri = check_orientation;
-    P.gridOrder = cur.take<uint16_t>((size_t)nf * P.maxFeat);
-    P.gridStart = cur.take<uint16_t>((size_t)nf * (GRID_COLS * GRID_ROWS + 1));
-    P.topk = cur.take<unsigned long long>((size_t)nq * PM_K);
-    P.cnt = cur.take<int>(nq);
-    P.quv = cur.take<float>(nq);
-    P.match = dev ? feature_match_out : cur.take<int>(total_rows);
-    P.nmatches = (dev && nmatches_out) ? nmatches_out : cur.take<int>(nf);
+    auto layout = [&](Carve& c) {
+        P.frame_image = stage_in(c, Q->frame_image, nf, dev); P.qoff = stage_in(c, Q->query_offset, nf + 1, dev);
+        P.Tcw = stage_in(c, Q->Tcw, (size_t)nf * 7, dev); P.direction = stage_in(c, Q->direction, nf, dev);
+        P.a0 = stage_in(c, Q->world_pos, (size_t)nq * 3, dev); P.level = stage_in(c, Q->last_octave, nq, dev);
+        P.f0 = stage_in(c, Q->last_angle, nq, dev); P.qdesc = stage_in(c, Q->desc, (size_t)nq * 32, dev);
+        P.flag = stage_in(c, Q->obs_positive, nq, dev);
+        P.gridOrder = c.take<uint16_t>((size_t)nf * P.maxFeat);
+        P.gridStart = c.take<uint16_t>((size_t)nf * (GRID_COLS * GRID_ROWS + 1));
+        P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
+        P.cnt = c.take<int>(nq);
+        P.quv = c.take<float>(nq);
+        P.match = dev ? feature_match_out : c.take<int>(total_rows);
+        P.nmatches = (dev && nmatches_out) ? nmatches_out : c.take<int>(nf);
+        P.seqFlag = c.take<int>(nf);
+    };
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     ORB_CUDA(cudaMemsetAsync(P.match, 0xff, sizeof(int) * (size_t)total_rows, h->stream));
-    P.seqFlag = cur.take<int>(nf);
     ORB_CUDA(cudaMemsetAsync(P.seqFlag, 0, sizeof(int) * nf, h->stream));
     if ((s = launch_proj(h, P, nf, maxq)) != ORB_OK) return s;
     if (!dev) {
@@ -1430,48 +1358,28 @@ extern "C" orb_status orbm_search_bow(orbx_handle* h, const orbm_bow_queries* Q,
     if (!h || !Q || !feature_match_out || Q->n_frames < 1 || !Q->frame_image || !Q->query_offset || !Q->feature_node)
         return set_error(ORB_ERR_INVALID, "bad arguments");
     ORB_CUDA(cudaSetDevice(h->cfg.device));
-    orb_status s = orbx_counts(h, nullptr, nullptr, nullptr);
-    if (s != ORB_OK) return s;
-    const int total_rows = h->h_counts[2 * h->cfg.max_batch + h->last_batch];
     const bool dev = Q->on_device != 0;
     const int nf = Q->n_frames;
-    std::vector<int> qoff_h(nf + 1), fimg_h(nf);
-    if (dev) {
-        ORB_CUDA(cudaMemcpyAsync(qoff_h.data(), Q->query_offset, sizeof(int) * (nf + 1), cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaMemcpyAsync(fimg_h.data(), Q->frame_image, sizeof(int) * nf, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-    } else {
-        std::copy(Q->query_offset, Q->query_offset + nf + 1, qoff_h.begin());
-        std::copy(Q->frame_image, Q->frame_image + nf, fimg_h.begin());
-    }
-    const int nq = qoff_h[nf];
-    int maxq = 0;
-    for (int f = 0; f < nf; ++f) {
-        maxq = std::max(maxq, qoff_h[f + 1] - qoff_h[f]);
-        if (fimg_h[f] < 0 || fimg_h[f] >= h->last_batch || qoff_h[f + 1] < qoff_h[f]) return set_error(ORB_ERR_INVALID, "bad frame table");
-    }
-    const size_t need = (size_t)nq * (PM_K * 8 + 4 + 4 + 4 + 4 + 32 + 16) + (size_t)total_rows * 8 + (size_t)nf * 64 + 65536;
-    if ((s = ensure_stage(h, need)) != ORB_OK) return s;
-    StageCursor cur{h->d_stage};
+    int nq, maxq, total_rows;
+    orb_status s = frame_table(h, nf, Q->frame_image, Q->query_offset, dev, false, nq, maxq, total_rows);
+    if (s != ORB_OK) return s;
     ProjParams P{};
     orbm_camera cam{1, 1, 0, 0, 0, 1, 0, (float)h->cur_w, 0, (float)h->cur_h};   // the grid is not used by this search
     fill_frame_side(h, &cam, P);
     P.uright = nullptr;
     P.mode = 2;
-    int *d_fimg, *d_qoff, *qnode, *fnode; float* ang; uint8_t* qd;
-    if ((s = upload(h, d_fimg, (const int*)Q->frame_image, nf, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, d_qoff, (const int*)Q->query_offset, nf + 1, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, qnode, (const int*)Q->query_node, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, ang, Q->query_angle, nq, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, qd, Q->desc, (size_t)nq * 32, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, fnode, (const int*)Q->feature_node, (size_t)total_rows, cur, dev)) != ORB_OK) return s;
-    P.frame_image = d_fimg; P.qoff = d_qoff; P.level = qnode; P.f0 = ang; P.qdesc = qd; P.feat_node = fnode;
     P.nnratio = nnratio; P.checkOri = check_orientation;
-    P.topk = cur.take<unsigned long long>((size_t)nq * PM_K);
-    P.cnt = cur.take<int>(std::max(nq, 1));
-    P.quv = cur.take<float>(std::max(nq, 1));
-    P.match = dev ? feature_match_out : cur.take<int>(std::max(total_rows, 1));
-    P.nmatches = (dev && nmatches_out) ? nmatches_out : cur.take<int>(nf);
+    auto layout = [&](Carve& c) {
+        P.frame_image = stage_in(c, Q->frame_image, nf, dev); P.qoff = stage_in(c, Q->query_offset, nf + 1, dev);
+        P.level = stage_in(c, Q->query_node, nq, dev); P.f0 = stage_in(c, Q->query_angle, nq, dev);
+        P.qdesc = stage_in(c, Q->desc, (size_t)nq * 32, dev); P.feat_node = stage_in(c, Q->feature_node, total_rows, dev);
+        P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
+        P.cnt = c.take<int>(nq);
+        P.quv = c.take<float>(nq);
+        P.match = dev ? feature_match_out : c.take<int>(total_rows);
+        P.nmatches = (dev && nmatches_out) ? nmatches_out : c.take<int>(nf);
+    };
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     ORB_CUDA(cudaMemsetAsync(P.match, 0xff, sizeof(int) * (size_t)total_rows, h->stream));
     if ((s = launch_proj(h, P, nf, maxq)) != ORB_OK) return s;
     if (!dev) {
@@ -1501,7 +1409,7 @@ extern "C" orb_status orbm_search_keyframe(orbx_handle* h, const orbm_camera* ca
         maxq = std::max(maxq, Q->query_offset[t + 1] - Q->query_offset[t]);
     }
     ProjParams P{};
-    size_t rows = 0;
+    int rows = 0;
     int maxFeat = 1;
     std::vector<int> img(nt), nkp(nt);
     orb_status s;
@@ -1513,61 +1421,45 @@ extern "C" orb_status orbm_search_keyframe(orbx_handle* h, const orbm_camera* ca
             nkp[t] = n;
             maxFeat = std::max(maxFeat, n);
         }
-        rows = (size_t)Q->feat_offset[nt];
+        rows = Q->feat_offset[nt];
     } else {
-        if ((s = orbx_counts(h, nullptr, nullptr, nullptr)) != ORB_OK) return s;
-        rows = (size_t)h->h_counts[2 * h->cfg.max_batch + h->last_batch];
+        if ((s = batch_rows(h, &rows)) != ORB_OK) return s;
         for (int t = 0; t < nt; ++t) {
             img[t] = Q->target_image[t];
             if (img[t] < 0 || img[t] >= h->last_batch) return set_error(ORB_ERR_INVALID, "bad target image");
         }
         maxFeat = h->geom.kpTotal;
     }
-    const size_t need = (size_t)nq * (PM_K * 8 + 4 + 4 + 12 + 12 + 8 + 32 + 4 + 4 + 64) + rows * (sizeof(orbx_keypoint) + 32 + 4 + 1) +
-                        (size_t)nt * (128 + 2 * (size_t)maxFeat + 2 * 3073 + 512) + 65536;
-    if ((s = ensure_stage(h, need)) != ORB_OK) return s;
-    StageCursor cur{h->d_stage};
     fill_frame_side(h, cam, P);
     P.mode = 3;
     P.variant = variant;
-    int *d_img, *d_qoff;
-    if ((s = upload(h, d_img, (const int*)img.data(), nt, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, d_qoff, (const int*)Q->query_offset, nt + 1, cur, false)) != ORB_OK) return s;
-    P.frame_image = d_img; P.qoff = d_qoff;
-    uint8_t* fl = nullptr;
-    if (Q->kp) {
-        orbx_keypoint* kp; uint8_t* de; float* ur; int *off, *nk;
-        if ((s = upload(h, kp, Q->kp, rows, cur, false)) != ORB_OK) return s;
-        if ((s = upload(h, de, Q->desc, rows * 32, cur, false)) != ORB_OK) return s;
-        if ((s = upload(h, ur, Q->uright, rows, cur, false)) != ORB_OK) return s;
-        if ((s = upload(h, off, (const int*)Q->feat_offset, nt, cur, false)) != ORB_OK) return s;
-        if ((s = upload(h, nk, (const int*)nkp.data(), nt, cur, false)) != ORB_OK) return s;
-        P.kps = kp; P.desc = de; P.uright = ur; P.offsets = off; P.nkp = nk; P.maxFeat = maxFeat;
-    }
-    if ((s = upload(h, fl, Q->feat_claimed, rows, cur, false)) != ORB_OK) return s;
-    float *tcw, *ow, *xw, *nr, *mx, *mn, *ang, *s8; uint8_t* qd;
-    if ((s = upload(h, s8, Q->Sim3, (size_t)nt * 8, cur, false)) != ORB_OK) return s;
-    P.S = s8;
-    if ((s = upload(h, tcw, Q->Tcw, (size_t)nt * 7, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, ow, Q->Ow, (size_t)nt * 3, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, xw, Q->world_pos, (size_t)nq * 3, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, nr, Q->normal, (size_t)nq * 3, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, mx, Q->max_dist, nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, mn, Q->min_dist, nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, ang, Q->angle, nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, qd, Q->desc_q, (size_t)nq * 32, cur, false)) != ORB_OK) return s;
-    P.Tcw = tcw; P.Ow = ow; P.a0 = xw; P.normal = nr; P.maxD = mx; P.minD = mn; P.f0 = ang; P.qdesc = qd; P.flag = fl;
+    if (Q->kp) P.maxFeat = maxFeat;
     P.th = th; P.thr = hamming_max; P.checkOri = (variant == 3) ? check_orientation : 0;
     P.nLevels = h->cfg.n_levels;
     P.logScale = logf((float)h->cfg.scale_factor);                       // Frame.cc:121 mfLogScaleFactor = log(mfScaleFactor)
     for (int l = 0; l < ORB_MAX_LEVELS; ++l) P.invSigma2[l] = l < h->cfg.n_levels ? h->inv_sigma2[l] : 1.f;
-    P.gridOrder = cur.take<uint16_t>((size_t)nt * P.maxFeat);
-    P.gridStart = cur.take<uint16_t>((size_t)nt * (GRID_COLS * GRID_ROWS + 1));
-    P.topk = cur.take<unsigned long long>((size_t)std::max(nq, 1) * PM_K);
-    P.cnt = cur.take<int>(std::max(nq, 1));
-    P.quv = cur.take<float>(std::max(nq, 1));
-    P.match = cur.take<int>(std::max(nq, 1));
-    P.nmatches = cur.take<int>(nt);
+    auto layout = [&](Carve& c) {
+        P.frame_image = stage_in(c, img.data(), nt, false); P.qoff = stage_in(c, Q->query_offset, nt + 1, false);
+        if (Q->kp) {
+            P.kps = stage_in(c, Q->kp, rows, false); P.desc = stage_in(c, Q->desc, (size_t)rows * 32, false);
+            P.uright = stage_in(c, Q->uright, rows, false); P.offsets = stage_in(c, Q->feat_offset, nt, false);
+            P.nkp = stage_in(c, nkp.data(), nt, false);
+        }
+        P.flag = stage_in(c, Q->feat_claimed, rows, false);
+        P.S = stage_in(c, Q->Sim3, (size_t)nt * 8, false);
+        P.Tcw = stage_in(c, Q->Tcw, (size_t)nt * 7, false); P.Ow = stage_in(c, Q->Ow, (size_t)nt * 3, false);
+        P.a0 = stage_in(c, Q->world_pos, (size_t)nq * 3, false); P.normal = stage_in(c, Q->normal, (size_t)nq * 3, false);
+        P.maxD = stage_in(c, Q->max_dist, nq, false); P.minD = stage_in(c, Q->min_dist, nq, false);
+        P.f0 = stage_in(c, Q->angle, nq, false); P.qdesc = stage_in(c, Q->desc_q, (size_t)nq * 32, false);
+        P.gridOrder = c.take<uint16_t>((size_t)nt * P.maxFeat);
+        P.gridStart = c.take<uint16_t>((size_t)nt * (GRID_COLS * GRID_ROWS + 1));
+        P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
+        P.cnt = c.take<int>(nq);
+        P.quv = c.take<float>(nq);
+        P.match = c.take<int>(nq);
+        P.nmatches = c.take<int>(nt);
+    };
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     if (nq > 0) {
         if ((s = launch_proj(h, P, nt, maxq)) != ORB_OK) return s;
         ORB_CUDA(cudaMemcpyAsync(match_out, P.match, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, h->stream));
@@ -1601,36 +1493,28 @@ extern "C" orb_status orbm_search_bow_keyframes(orbx_handle* h, const orbm_bow_k
     std::vector<uint8_t> invalid(std::max<size_t>(rows, 1), 0);   // vbMatched2 starts false; features without a good map point never match
     if (Q->valid2)
         for (size_t i = 0; i < rows; ++i) invalid[i] = Q->valid2[i] ? 0 : 1;
-    const size_t need = (size_t)nq * (PM_K * 8 + 4 + 4 + 4 + 4 + 32 + 64) + rows * (sizeof(orbx_keypoint) + 32 + 4 + 1) + (size_t)nt * 128 + 65536;
-    orb_status s;
-    if ((s = ensure_stage(h, need)) != ORB_OK) return s;
-    StageCursor cur{h->d_stage};
     ProjParams P{};
     orbm_camera cam{1, 1, 0, 0, 0, 1, 0, 1, 0, 1};   // the grid is not used by this search
     fill_frame_side(h, &cam, P);
     P.mode = 2;
     P.variant = 1;
-    int *d_img, *d_qoff, *off, *nk, *qnode, *fnode; orbx_keypoint* kp; uint8_t *de, *fl, *qd; float* ang;
-    if ((s = upload(h, d_img, (const int*)img.data(), nt, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, d_qoff, (const int*)Q->query_offset, nt + 1, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, kp, Q->kp2, rows, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, de, Q->desc2, rows * 32, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, off, (const int*)Q->feat_offset, nt, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, nk, (const int*)nkp.data(), nt, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, fnode, (const int*)Q->node2, rows, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, fl, (const uint8_t*)invalid.data(), rows, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, qnode, (const int*)Q->query_node, nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, ang, Q->query_angle, nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, qd, Q->desc1, (size_t)nq * 32, cur, false)) != ORB_OK) return s;
-    P.frame_image = d_img; P.qoff = d_qoff;
-    P.kps = kp; P.desc = de; P.uright = nullptr; P.offsets = off; P.nkp = nk; P.maxFeat = maxFeat;
-    P.feat_node = fnode; P.flag = fl; P.level = qnode; P.f0 = ang; P.qdesc = qd;
+    P.uright = nullptr; P.maxFeat = maxFeat;
     P.nnratio = nnratio; P.checkOri = check_orientation;
-    P.topk = cur.take<unsigned long long>((size_t)std::max(nq, 1) * PM_K);
-    P.cnt = cur.take<int>(std::max(nq, 1));
-    P.quv = cur.take<float>(std::max(nq, 1));
-    P.match = cur.take<int>(std::max(nq, 1));
-    P.nmatches = cur.take<int>(nt);
+    auto layout = [&](Carve& c) {
+        P.frame_image = stage_in(c, img.data(), nt, false); P.qoff = stage_in(c, Q->query_offset, nt + 1, false);
+        P.kps = stage_in(c, Q->kp2, rows, false); P.desc = stage_in(c, Q->desc2, rows * 32, false);
+        P.offsets = stage_in(c, Q->feat_offset, nt, false); P.nkp = stage_in(c, nkp.data(), nt, false);
+        P.feat_node = stage_in(c, Q->node2, rows, false); P.flag = stage_in(c, invalid.data(), rows, false);
+        P.level = stage_in(c, Q->query_node, nq, false); P.f0 = stage_in(c, Q->query_angle, nq, false);
+        P.qdesc = stage_in(c, Q->desc1, (size_t)nq * 32, false);
+        P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
+        P.cnt = c.take<int>(nq);
+        P.quv = c.take<float>(nq);
+        P.match = c.take<int>(nq);
+        P.nmatches = c.take<int>(nt);
+    };
+    orb_status s;
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     if (nq > 0) {
         if ((s = launch_proj(h, P, nt, maxq)) != ORB_OK) return s;
         ORB_CUDA(cudaMemcpyAsync(match12_out, P.match, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, h->stream));
@@ -1669,40 +1553,31 @@ extern "C" orb_status orbm_search_initialization(orbx_handle* h, const orbm_came
         lvl[i] = Q->kp1[i].octave;
     }
     const int qoff_h[2] = {0, nq};
-    const size_t need = (size_t)nq * (PM_K * 8 + 4 * 8 + 32 + 64) + rows * (sizeof(orbx_keypoint) + 32 + 8) +
-                        2 * (size_t)std::max(h->geom.kpTotal, (int)rows) + 2 * 3073 + 65536;
-    if ((s = ensure_stage(h, need)) != ORB_OK) return s;
-    StageCursor cur{h->d_stage};
     ProjParams P{};
     fill_frame_side(h, cam, P);
     P.uright = nullptr;
     P.mode = 4;
-    int *d_img, *d_qoff, *d_lvl; float *d_px, *d_py, *d_ang; uint8_t* qd;
-    if ((s = upload(h, d_img, (const int*)&img, 1, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, d_qoff, (const int*)qoff_h, 2, cur, false)) != ORB_OK) return s;
-    if (Q->kp2) {
-        orbx_keypoint* kp; uint8_t* de; int *off, *nk;
-        if ((s = upload(h, kp, Q->kp2, rows, cur, false)) != ORB_OK) return s;
-        if ((s = upload(h, de, Q->desc2, rows * 32, cur, false)) != ORB_OK) return s;
-        if ((s = upload(h, off, (const int*)&off_h, 1, cur, false)) != ORB_OK) return s;
-        if ((s = upload(h, nk, (const int*)&nkp_h, 1, cur, false)) != ORB_OK) return s;
-        P.kps = kp; P.desc = de; P.offsets = off; P.nkp = nk; P.maxFeat = std::max(Q->n2, 1);
-    }
-    if ((s = upload(h, d_px, (const float*)px.data(), nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, d_py, (const float*)py.data(), nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, d_ang, (const float*)ang.data(), nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, d_lvl, (const int*)lvl.data(), nq, cur, false)) != ORB_OK) return s;
-    if ((s = upload(h, qd, Q->desc1, (size_t)nq * 32, cur, false)) != ORB_OK) return s;
-    P.frame_image = d_img; P.qoff = d_qoff; P.a0 = d_px; P.a1 = d_py; P.f0 = d_ang; P.level = d_lvl; P.qdesc = qd;
+    if (Q->kp2) P.maxFeat = std::max(Q->n2, 1);
     P.th = (float)window_size;     // GetFeaturesInArea(x, y, windowSize, ...): int -> const float& r
     P.nnratio = nnratio; P.checkOri = check_orientation;
-    P.gridOrder = cur.take<uint16_t>((size_t)P.maxFeat);
-    P.gridStart = cur.take<uint16_t>((size_t)(GRID_COLS * GRID_ROWS + 1));
-    P.topk = cur.take<unsigned long long>((size_t)std::max(nq, 1) * PM_K);
-    P.cnt = cur.take<int>(std::max(nq, 1));
-    P.quv = cur.take<float>(std::max(nq, 1));
-    P.match = cur.take<int>(std::max(nq, 1));
-    P.nmatches = cur.take<int>(1);
+    auto layout = [&](Carve& c) {
+        P.frame_image = stage_in(c, &img, 1, false); P.qoff = stage_in(c, qoff_h, 2, false);
+        if (Q->kp2) {
+            P.kps = stage_in(c, Q->kp2, rows, false); P.desc = stage_in(c, Q->desc2, rows * 32, false);
+            P.offsets = stage_in(c, &off_h, 1, false); P.nkp = stage_in(c, &nkp_h, 1, false);
+        }
+        P.a0 = stage_in(c, px.data(), nq, false); P.a1 = stage_in(c, py.data(), nq, false);
+        P.f0 = stage_in(c, ang.data(), nq, false); P.level = stage_in(c, lvl.data(), nq, false);
+        P.qdesc = stage_in(c, Q->desc1, (size_t)nq * 32, false);
+        P.gridOrder = c.take<uint16_t>((size_t)P.maxFeat);
+        P.gridStart = c.take<uint16_t>((size_t)(GRID_COLS * GRID_ROWS + 1));
+        P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
+        P.cnt = c.take<int>(nq);
+        P.quv = c.take<float>(nq);
+        P.match = c.take<int>(nq);
+        P.nmatches = c.take<int>(1);
+    };
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     if (nq > 0) {
         if ((s = launch_proj(h, P, 1, nq)) != ORB_OK) return s;
         ORB_CUDA(cudaMemcpyAsync(matches12_out, P.match, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, h->stream));
@@ -1733,34 +1608,27 @@ extern "C" orb_status orbf_is_in_frustum(orbx_handle* h, const orbm_camera* cam,
         }
     }
     if (np > 0 && (!in->world_pos || !in->normal || !in->max_dist || !in->min_dist)) return set_error(ORB_ERR_INVALID, "missing point arrays");
-    orb_status s;
-    const size_t need = dev ? 4096 : (size_t)np * (12 + 12 + 4 + 4 + 1 + 4 * 5 + 4 + 64) + (size_t)nf * 128 + 65536;
-    if ((s = ensure_stage(h, need)) != ORB_OK) return s;
-    StageCursor cur{h->d_stage};
     FrustumParams P{};
-    int* poff; float *R, *t, *O, *xw, *nr, *mx, *mn;
-    if ((s = upload(h, poff, (const int*)in->point_offset, nf + 1, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, R, in->Rcw, (size_t)nf * 9, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, t, in->tcw, (size_t)nf * 3, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, O, in->Ow, (size_t)nf * 3, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, xw, in->world_pos, (size_t)np * 3, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, nr, in->normal, (size_t)np * 3, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, mx, in->max_dist, np, cur, dev)) != ORB_OK) return s;
-    if ((s = upload(h, mn, in->min_dist, np, cur, dev)) != ORB_OK) return s;
-    P.poff = poff; P.Rcw = R; P.tcw = t; P.Ow = O; P.xw = xw; P.normal = nr; P.maxD = mx; P.minD = mn;
     P.fx = cam->fx; P.fy = cam->fy; P.cx = cam->cx; P.cy = cam->cy; P.bf = cam->bf;
     P.minX = cam->min_x; P.maxX = cam->max_x; P.minY = cam->min_y; P.maxY = cam->max_y;
     P.logScale = logf((float)h->cfg.scale_factor);
     P.cosLimit = viewing_cos_limit;
     P.nLevels = h->cfg.n_levels;
-    const int npa = std::max(np, 1);
-    P.in_view = dev ? in_view_out : cur.take<uint8_t>(npa);
-    P.px = dev ? proj_x_out : cur.take<float>(npa);
-    P.py = dev ? proj_y_out : cur.take<float>(npa);
-    P.pxr = dev ? proj_xr_out : cur.take<float>(npa);
-    P.vc = dev ? view_cos_out : cur.take<float>(npa);
-    P.depth = dev ? track_depth_out : cur.take<float>(npa);
-    P.level = dev ? level_out : cur.take<int>(npa);
+    auto layout = [&](Carve& c) {
+        P.poff = stage_in(c, in->point_offset, nf + 1, dev); P.Rcw = stage_in(c, in->Rcw, (size_t)nf * 9, dev);
+        P.tcw = stage_in(c, in->tcw, (size_t)nf * 3, dev); P.Ow = stage_in(c, in->Ow, (size_t)nf * 3, dev);
+        P.xw = stage_in(c, in->world_pos, (size_t)np * 3, dev); P.normal = stage_in(c, in->normal, (size_t)np * 3, dev);
+        P.maxD = stage_in(c, in->max_dist, np, dev); P.minD = stage_in(c, in->min_dist, np, dev);
+        P.in_view = dev ? in_view_out : c.take<uint8_t>(np);
+        P.px = dev ? proj_x_out : c.take<float>(np);
+        P.py = dev ? proj_y_out : c.take<float>(np);
+        P.pxr = dev ? proj_xr_out : c.take<float>(np);
+        P.vc = dev ? view_cos_out : c.take<float>(np);
+        P.depth = dev ? track_depth_out : c.take<float>(np);
+        P.level = dev ? level_out : c.take<int>(np);
+    };
+    orb_status s;
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     if (maxp > 0) {
         k_in_frustum<<<dim3((maxp + 255) / 256, nf), 256, 0, h->stream>>>(P);
         ORB_LAUNCHED();

@@ -356,18 +356,6 @@ __global__ void __launch_bounds__(PE_THREADS) k_pose_edges(const __grid_constant
 
 }  // namespace orb
 
-struct PoStage {
-    uint8_t* base;
-    size_t off = 0;
-    template <typename T>
-    T* take(size_t n) {
-        off = (off + 255) / 256 * 256;
-        T* p = reinterpret_cast<T*>(base + off);
-        off += n * sizeof(T);
-        return p;
-    }
-};
-
 extern "C" orb_status orbo_pose_optimization(orbx_handle* h, const orbo_pose_problems* in, double* pose_out, uint8_t* outlier_out,
                                              int32_t* inliers_out, int32_t* stats_out) {
     if (!h || !in || in->n_frames < 1 || !in->edge_offset || !in->pose || !pose_out || !inliers_out)
@@ -379,39 +367,20 @@ extern "C" orb_status orbo_pose_optimization(orbx_handle* h, const orbo_pose_pro
     const int ne = dev ? in->n_edges_max : in->edge_offset[nf];
     if (ne < 0 || (ne > 0 && (!in->world_pos || !in->obs || !in->inv_sigma2 || !outlier_out))) return set_error(ORB_ERR_INVALID, "missing edge arrays");
     // scratch (and, for host callers, staging) comes from the handle's matcher stage buffer
-    const size_t need = (size_t)ne * (8 + 1 + (dev ? 0 : 28)) + (size_t)nf * (dev ? 16 : 128) + 65536;
-    if (need > h->stage_bytes) {
-        if (h->d_stage) cudaFree(h->d_stage);
-        h->d_stage = nullptr;
-        h->stage_bytes = 0;
-        const size_t want = (need + (1 << 20)) / (1 << 20) * (1 << 20);
-        ORB_CUDA(cudaMalloc((void**)&h->d_stage, want));
-        h->stage_bytes = want;
-    }
-    PoStage cur{h->d_stage};
     PoseOptParams P{};
     P.fx = in->fx; P.fy = in->fy; P.cx = in->cx; P.cy = in->cy; P.bf = in->bf;   // float members promoted (Optimizer.cc:146-150)
-    P.err = cur.take<double>(std::max(ne, 1));
-    auto up = [&](auto*& dst, const auto* src, size_t n) -> orb_status {
-        using T = std::remove_cv_t<std::remove_pointer_t<decltype(src)>>;
-        if (dev) { dst = const_cast<T*>(src); return ORB_OK; }
-        T* d = cur.take<T>(std::max<size_t>(n, 1));
-        if (n) ORB_CUDA(cudaMemcpyAsync(d, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
-        dst = d;
-        return ORB_OK;
+    auto layout = [&](Carve& c) {
+        P.err = c.take<double>(ne);
+        P.eoff = stage_in(c, in->edge_offset, nf + 1, dev); P.pose = stage_in(c, in->pose, (size_t)nf * 7, dev);
+        P.xw = stage_in(c, in->world_pos, (size_t)ne * 3, dev); P.obs = stage_in(c, in->obs, (size_t)ne * 3, dev);
+        P.invs2 = stage_in(c, in->inv_sigma2, ne, dev);
+        P.outlier = dev ? outlier_out : c.take<uint8_t>(ne);
+        P.pose_out = dev ? pose_out : c.take<double>((size_t)nf * 7);
+        P.inliers = dev ? inliers_out : c.take<int>(nf);
+        P.stats = (dev && stats_out) ? stats_out : c.take<int>((size_t)nf * 4);
     };
-    int* eoff; float *pose, *xw, *obs, *w;
-    orb_status s;
-    if ((s = up(eoff, (const int*)in->edge_offset, nf + 1)) != ORB_OK) return s;
-    if ((s = up(pose, in->pose, (size_t)nf * 7)) != ORB_OK) return s;
-    if ((s = up(xw, in->world_pos, (size_t)ne * 3)) != ORB_OK) return s;
-    if ((s = up(obs, in->obs, (size_t)ne * 3)) != ORB_OK) return s;
-    if ((s = up(w, in->inv_sigma2, (size_t)ne)) != ORB_OK) return s;
-    P.eoff = eoff; P.pose = pose; P.xw = xw; P.obs = obs; P.invs2 = w;
-    P.outlier = dev ? outlier_out : cur.take<uint8_t>(std::max(ne, 1));
-    P.pose_out = dev ? pose_out : cur.take<double>((size_t)nf * 7);
-    P.inliers = dev ? inliers_out : cur.take<int>(nf);
-    P.stats = (dev && stats_out) ? stats_out : cur.take<int>((size_t)nf * 4);
+    const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (s != ORB_OK) return s;
     k_pose_opt<<<nf, PO_THREADS, 0, h->stream>>>(P);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
@@ -434,14 +403,6 @@ extern "C" orb_status orbo_pose_edges(orbx_handle* h, const orbo_edge_source* sr
     if (h->last_batch < 1) return set_error(ORB_ERR_INVALID, "no batch has been extracted");
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     const int nf = src->n_frames;
-    const size_t need = (size_t)nf * 4 + 4096;
-    if (need > h->stage_bytes) {
-        if (h->d_stage) cudaFree(h->d_stage);
-        h->d_stage = nullptr;
-        h->stage_bytes = 0;
-        ORB_CUDA(cudaMalloc((void**)&h->d_stage, (size_t)1 << 20));
-        h->stage_bytes = (size_t)1 << 20;
-    }
     EdgeParams P{};
     P.kps = h->d_kps; P.uright = h->stereo_valid ? h->d_uright : nullptr; P.offsets = h->d_offsets; P.nkp = h->d_nkp;
     P.maxFeat = h->geom.kpTotal;
@@ -449,7 +410,8 @@ extern "C" orb_status orbo_pose_edges(orbx_handle* h, const orbo_edge_source* sr
     P.xw = src->world_pos;
     P.xw2 = src->query_world_pos;
     for (int l = 0; l < ORB_MAX_LEVELS; ++l) P.invSigma2[l] = l < h->cfg.n_levels ? h->inv_sigma2[l] : 1.f;
-    P.cnt = reinterpret_cast<int*>(h->d_stage);
+    const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, [&](Carve& c) { P.cnt = c.take<int>(nf); });
+    if (s != ORB_OK) return s;
     P.eoff = edge_offset_out; P.efeat = edge_feature_out; P.exw = world_pos_out; P.eobs = obs_out; P.ew = inv_sigma2_out;
     const size_t sm = (size_t)P.maxFeat * 4;
     k_pose_edges<false><<<nf, PE_THREADS, sm, h->stream>>>(P, nf);
@@ -466,10 +428,10 @@ extern "C" orb_status orbo_pose_optimization_frames(orbx_handle* h, const orbo_f
         ((in->feature_match != nullptr) == (in->query_match != nullptr)) || (in->query_match && !in->query_offset) || !pose_out || !inliers_out)
         return set_error(ORB_ERR_INVALID, "bad arguments");
     ORB_CUDA(cudaSetDevice(h->cfg.device));
-    orb_status s = orbx_counts(h, nullptr, nullptr, nullptr);
+    int total_rows = 0;
+    orb_status s = batch_rows(h, &total_rows);
     if (s != ORB_OK) return s;
     const int nf = in->n_frames, MB = h->cfg.max_batch;
-    const int total_rows = h->h_counts[2 * MB + h->last_batch];
     size_t cap = 0;                               // edges <= features of the listed frames
     for (int f = 0; f < nf; ++f) {
         const int img = in->frame_image[f];
@@ -478,42 +440,19 @@ extern "C" orb_status orbo_pose_optimization_frames(orbx_handle* h, const orbo_f
     }
     cap = std::max<size_t>(cap, 1);
     const int nq = in->n_queries;
-    const size_t need = (size_t)nf * (4 * 4 + 7 * 4 + 7 * 8 + 64) + cap * (4 + 12 + 12 + 4 + 1 + 64) + (size_t)nq * (12 + 4) + (size_t)total_rows * 4 + 65536;
-    if (need > h->po_bytes) {
-        if (h->d_po) cudaFree(h->d_po);
-        h->d_po = nullptr;
-        h->po_bytes = 0;
-        const size_t want = (need + (1 << 20)) / (1 << 20) * (1 << 20);
-        ORB_CUDA(cudaMalloc((void**)&h->d_po, want));
-        h->po_bytes = want;
-    }
-    PoStage cur{h->d_po};
+    const int nqm = in->query_match ? in->query_offset[nf] : 0;
     cudaStream_t st = h->stream;
-    auto up = [&](auto*& dst, const auto* src, size_t n) -> orb_status {
-        using T = std::remove_cv_t<std::remove_pointer_t<decltype(src)>>;
-        T* d = cur.take<T>(std::max<size_t>(n, 1));
-        if (n && src) ORB_CUDA(cudaMemcpyAsync(d, src, n * sizeof(T), cudaMemcpyHostToDevice, st));
-        dst = d;
-        return ORB_OK;
+    orbo_edge_source src{nf};
+    int *d_eoff, *d_efeat, *d_inl; float *d_pose, *d_exw, *d_eobs, *d_ew; double* d_pout; uint8_t* d_out;
+    auto layout = [&](Carve& c) {
+        src.frame_image = stage_in(c, in->frame_image, nf, false); d_pose = stage_in(c, in->pose, (size_t)nf * 7, false);
+        src.world_pos = stage_in(c, in->world_pos, (size_t)nq * 3, false);
+        src.feature_match = stage_in(c, in->feature_match, total_rows, false);
+        if (in->query_match) { src.query_offset = stage_in(c, in->query_offset, nf + 1, false); src.query_match = stage_in(c, in->query_match, nqm, false); }
+        d_eoff = c.take<int>(nf + 1); d_efeat = c.take<int>(cap); d_exw = c.take<float>(cap * 3); d_eobs = c.take<float>(cap * 3);
+        d_ew = c.take<float>(cap); d_pout = c.take<double>((size_t)nf * 7); d_out = c.take<uint8_t>(cap); d_inl = c.take<int>(nf);
     };
-    int *d_img, *d_fm = nullptr, *d_qoff = nullptr, *d_qm = nullptr; float *d_pose, *d_xw;
-    if ((s = up(d_img, (const int*)in->frame_image, nf)) != ORB_OK) return s;
-    if ((s = up(d_pose, in->pose, (size_t)nf * 7)) != ORB_OK) return s;
-    if ((s = up(d_xw, in->world_pos, (size_t)nq * 3)) != ORB_OK) return s;
-    if (in->feature_match) { if ((s = up(d_fm, (const int*)in->feature_match, (size_t)total_rows)) != ORB_OK) return s; }
-    else {
-        if ((s = up(d_qoff, (const int*)in->query_offset, nf + 1)) != ORB_OK) return s;
-        if ((s = up(d_qm, (const int*)in->query_match, (size_t)in->query_offset[nf])) != ORB_OK) return s;
-    }
-    int* d_eoff = cur.take<int>(nf + 1);
-    int* d_efeat = cur.take<int>(cap);
-    float* d_exw = cur.take<float>(cap * 3);
-    float* d_eobs = cur.take<float>(cap * 3);
-    float* d_ew = cur.take<float>(cap);
-    double* d_pout = cur.take<double>((size_t)nf * 7);
-    uint8_t* d_out = cur.take<uint8_t>(cap);
-    int* d_inl = cur.take<int>(nf);
-    orbo_edge_source src{nf, d_img, d_fm, d_qoff, d_qm, d_xw, nullptr};
+    if ((s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout)) != ORB_OK) return s;
     if ((s = orbo_pose_edges(h, &src, d_eoff, d_efeat, d_exw, d_eobs, d_ew)) != ORB_OK) return s;
     orbo_pose_problems pp{nf, 1, d_eoff, d_pose, d_exw, d_eobs, d_ew, in->fx, in->fy, in->cx, in->cy, in->bf, (int32_t)cap};
     if ((s = orbo_pose_optimization(h, &pp, d_pout, d_out, d_inl, nullptr)) != ORB_OK) return s;

@@ -41,20 +41,6 @@ struct orbr_state {
     int* d_clevel = nullptr;
 };
 
-namespace {
-struct Carve {
-    uint8_t* base;
-    size_t off = 0;
-    template <typename T>
-    T* take(size_t n) {
-        off = (off + 255) / 256 * 256;
-        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-        off += std::max<size_t>(n, 1) * sizeof(T);
-        return p;
-    }
-};
-}  // namespace
-
 
 // ---- the chained flow's glue kernels -------------------------------------------------------------------------------------
 namespace orb {
@@ -177,15 +163,14 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     }
     const size_t rows_cap = h->out_rows;   // compact rows a batch of max_batch images can produce
     const bool po = S->pose_optimization != 0 || CH != nullptr;
-    // ---- carve the step's device block (two passes: size, then pointers) ----
+    // ---- carve the step's device block ----
     struct Ptrs {
         int *fimgL, *qoffL, *dirL, *octL; float *tcwL, *xwL, *angL; uint8_t *descL, *obsL;
         int *fimgC, *qoffC, *lvlC; float *pxC, *pyC, *pxrC, *vcC, *tdC, *xwC; uint8_t *descC, *claimC, *viewC;
         float* pose;
         float *nrmK, *mxK, *mnK, *RcwK, *tcwK, *OwK; int* lastqK; uint8_t* seenK;
     } D{};
-    auto carve = [&](uint8_t* base) -> size_t {
-        Carve c{base};
+    auto layout = [&](Carve& c) {
         D.fimgL = c.take<int>(nf); D.qoffL = c.take<int>(nf + 1); D.dirL = c.take<int>(nf); D.tcwL = c.take<float>((size_t)nf * 7);
         D.xwL = c.take<float>((size_t)nqL * 3); D.octL = c.take<int>(nqL); D.angL = c.take<float>(nqL); D.descL = c.take<uint8_t>((size_t)nqL * 32);
         D.obsL = c.take<uint8_t>(nqL);
@@ -205,18 +190,9 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         D.seenK = c.take<uint8_t>(CH ? (size_t)nqL : 0);
         r->d_cview = c.take<uint8_t>(npK); r->d_cpx = c.take<float>(npK); r->d_cpy = c.take<float>(npK); r->d_cpxr = c.take<float>(npK);
         r->d_clevel = c.take<int>(npK); r->d_cvc = c.take<float>(npK); r->d_cdepth = c.take<float>(npK); r->d_posef = c.take<float>((size_t)nf * 7);
-        return c.off + 256;
     };
-    const size_t need = carve(nullptr);
-    if (need > r->bytes) {
-        if (r->d_buf) cudaFree(r->d_buf);
-        r->d_buf = nullptr;
-        r->bytes = 0;
-        const size_t want = (need + need / 4 + (1 << 20)) / (1 << 20) * (1 << 20);
-        ORB_CUDA(cudaMalloc((void**)&r->d_buf, want));
-        r->bytes = want;
-    }
-    carve(r->d_buf);
+    orb_status s = carve_scratch(r->bytes, r->d_buf, h->capturing, h->stream, layout);
+    if (s != ORB_OK) return s;
     if (r->h_eoff_cap < 2 * (nf + 1)) {
         if (r->h_eoff) cudaFreeHost(r->h_eoff);
         r->h_eoff = nullptr;
@@ -225,7 +201,7 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     }
     cudaStream_t st = h->stream;
     // ---- both eyes of every frame through the extractor, then ComputeStereoMatches ----
-    orb_status s = orbx_extract_batch(h, S->images, 2 * nf, S->width, S->height, S->stride, S->image_stride_bytes, 0, 0, nullptr, nullptr);
+    s = orbx_extract_batch(h, S->images, 2 * nf, S->width, S->height, S->stride, S->image_stride_bytes, 0, 0, nullptr, nullptr);
     if (s != ORB_OK) return s;
     if ((s = orbm_stereo_batch(h, nf, S->bf, S->b)) != ORB_OK) return s;
     auto up = [&](void* dst, const void* src, size_t bytes) -> orb_status {

@@ -341,9 +341,9 @@ extern "C" orb_status orbm_stereo_batch(orbx_handle* h, int32_t n_pairs, float b
 }
 
 extern "C" orb_status orbm_stereo_download(orbx_handle* h, float* uright, float* depth, int32_t cap_rows) {
-    orb_status s = orbx_counts(h, nullptr, nullptr, nullptr);
+    int total = 0;
+    orb_status s = batch_rows(h, &total);
     if (s != ORB_OK) return s;
-    const int total = h->h_counts[2 * h->cfg.max_batch + h->last_batch];
     const int rows = std::min(total, (int)cap_rows);
     if (rows > 0) {
         if (uright) ORB_CUDA(cudaMemcpyAsync(uright, h->d_uright, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));

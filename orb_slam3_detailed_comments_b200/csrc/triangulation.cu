@@ -164,32 +164,10 @@ extern "C" orb_status orbm_search_triangulation(orbx_handle* h, const orbm_trian
         for (int i = 0; i < nq; ++i) match12_out[i] = -1;
         return ORB_OK;
     }
-    const size_t need = (size_t)nq * (28 + 32 + 4 + 1 + 8) + (size_t)N2 * (28 + 32 + 4 + 2) + 65536;
-    if (need > h->stage_bytes) {
-        if (h->d_stage) cudaFree(h->d_stage);
-        h->d_stage = nullptr; h->stage_bytes = 0;
-        const size_t want = (need + (1 << 20)) / (1 << 20) * (1 << 20);
-        ORB_CUDA(cudaMalloc((void**)&h->d_stage, want));
-        h->stage_bytes = want;
-    }
-    size_t off = 0;
-    auto take = [&](size_t bytes) { off = (off + 255) / 256 * 256; uint8_t* p = h->d_stage + off; off += bytes; return p; };
-    auto up = [&](const void* src, size_t bytes) -> uint8_t* {
-        uint8_t* d = take(bytes);
-        cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, h->stream);
-        return d;
-    };
+    if (!T->kp1 || !T->desc1 || !T->node1 || !T->stereo1 || !T->kp2 || !T->desc2 || !T->node2 || !T->valid2 || !T->stereo2)
+        return set_error(ORB_ERR_INVALID, "missing triangulation arrays");
     TriParams P{};
     P.nq = nq; P.N2 = N2;
-    P.kp1 = (const orbx_keypoint*)up(T->kp1, (size_t)nq * sizeof(orbx_keypoint));
-    P.desc1 = up(T->desc1, (size_t)nq * 32);
-    P.node1 = (const int*)up(T->node1, (size_t)nq * 4);
-    P.stereo1 = up(T->stereo1, nq);
-    P.kp2 = (const orbx_keypoint*)up(T->kp2, (size_t)N2 * sizeof(orbx_keypoint));
-    P.desc2 = up(T->desc2, (size_t)N2 * 32);
-    P.node2 = (const int*)up(T->node2, (size_t)N2 * 4);
-    P.valid2 = up(T->valid2, N2);
-    P.stereo2 = up(T->stereo2, N2);
     for (int i = 0; i < 9; ++i) P.F12[i] = T->F12[i];
     P.ep[0] = T->epipole2[0]; P.ep[1] = T->epipole2[1];
     for (int l = 0; l < ORB_MAX_LEVELS; ++l) {
@@ -197,9 +175,17 @@ extern "C" orb_status orbm_search_triangulation(orbx_handle* h, const orbm_trian
         P.sigma2[l] = l < h->cfg.n_levels ? h->sigma2[l] : 1.f;
     }
     P.coarse = T->coarse; P.checkOri = T->check_orientation;
-    P.match = (int*)take((size_t)nq * 4);
-    P.bins = (int*)take((size_t)nq * 4);
-    P.nmatches = (int*)take(64);
+    auto layout = [&](Carve& c) {
+        P.kp1 = stage_in(c, T->kp1, nq, false); P.desc1 = stage_in(c, T->desc1, (size_t)nq * 32, false);
+        P.node1 = stage_in(c, T->node1, nq, false); P.stereo1 = stage_in(c, T->stereo1, nq, false);
+        P.kp2 = stage_in(c, T->kp2, N2, false); P.desc2 = stage_in(c, T->desc2, (size_t)N2 * 32, false);
+        P.node2 = stage_in(c, T->node2, N2, false); P.valid2 = stage_in(c, T->valid2, N2, false); P.stereo2 = stage_in(c, T->stereo2, N2, false);
+        P.match = c.take<int>(nq);
+        P.bins = c.take<int>(nq);
+        P.nmatches = c.take<int>(1);
+    };
+    const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (s != ORB_OK) return s;
     const size_t smem = (size_t)N2 * 14 + 16;
     ORB_CUDA(cudaFuncSetAttribute(k_tri_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem, (size_t)1024)));
     k_tri_match<<<(nq + TRI_QPB - 1) / TRI_QPB, TRI_WARPS * 32, smem, h->stream>>>(P);
