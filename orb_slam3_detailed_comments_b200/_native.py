@@ -16,6 +16,10 @@ SOURCES = ["extractor.cu", "stereo.cu", "matcher.cu", "triangulation.cu", "lba.c
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
+# k_blur_mma (the tensor-core blur) is its own library next to the main one, which links it and finds it through RUNPATH $ORIGIN
+BLUR_SOURCES = ["blur_mma.cu"]
+BLUR_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_blur.so")
+LINK_FLAGS = ["-L", os.path.dirname(BLUR_LIB_PATH), "-lorbslam3_b200_blur", "-Xlinker", "-rpath,$ORIGIN"]
 
 KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"),
                      ("response", "<f4"), ("octave", "<i4"), ("class_id", "<i4")])
@@ -26,18 +30,19 @@ class OrbError(RuntimeError):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so (nvcc cross-compiles on CPU)."""
-    srcs = [os.path.join(_CSRC, s) for s in SOURCES]
+    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200_blur.so and lib/liborbslam3_b200.so, which links the first
+    (nvcc cross-compiles on CPU)."""
     deps = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)] + [os.path.join(_PKG, "..", "include", "orbslam3_b200.h")]
     if os.environ.get("ORB_LIB_PATH"):
         return LIB_PATH                       # an explicitly chosen build is never rebuilt
-    if (not force and os.path.exists(LIB_PATH)
-            and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps)):
-        return LIB_PATH
-    os.makedirs(os.path.dirname(LIB_PATH), exist_ok=True)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB_PATH] + srcs
-    subprocess.check_call(cmd)
+    os.makedirs(os.path.dirname(LIB_PATH), exist_ok=True)
+    for out, sources, link in [(BLUR_LIB_PATH, BLUR_SOURCES, []), (LIB_PATH, SOURCES, LINK_FLAGS)]:
+        if (not force and os.path.exists(out)
+                and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps)):
+            continue
+        cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", out] + [os.path.join(_CSRC, s) for s in sources] + link
+        subprocess.check_call(cmd)
     return LIB_PATH
 
 

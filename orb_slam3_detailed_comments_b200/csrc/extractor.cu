@@ -11,6 +11,7 @@
 
 #include "extractor.h"
 #include "extractor_kernels.cuh"
+#include "blur_mma.cuh"
 
 namespace orb {
 thread_local std::string g_last_error;
@@ -320,7 +321,7 @@ extern "C" orb_status orbx_create(const orbx_config* cfg, orbx_handle** out) {
     h->cfg = *cfg;
     if (const char* v = getenv("ORB_FAST_VARIANT")) h->fast_variant = atoi(v) == 0 ? 0 : 1;   // 0 selects the round-1 kernel
     if (const char* v = getenv("ORB_QT_VARIANT")) h->qt_variant = atoi(v) == 0 ? 0 : 1;   // 0 selects the round-1 kernel (k_quadtree)
-    if (const char* v = getenv("ORB_BLUR_VARIANT")) h->blur_variant = atoi(v);       // 0: packed 16x2 multiply-adds instead of IDP.4A
+    if (const char* v = getenv("ORB_BLUR_VARIANT")) h->blur_variant = atoi(v);       // 1: k_blur<true> (IDP.4A), 0: k_blur<false> (packed 16x2 multiply-adds)
     if (const char* v = getenv("ORB_RESIZE_VARIANT")) h->resize_variant = atoi(v);   // 0: k_resize (4 px of one row per thread)
     if (const char* v = getenv("ORB_FAST_TMA")) h->fast_tma = atoi(v) != 0;   // window rows of k_fast_cells_v2 staged by TMA bulk copies
     if (const char* v = getenv("ORB_QT_GROUPS")) h->qt_max_groups = atoi(v) == 4 ? 4 : 3;
@@ -379,7 +380,14 @@ extern "C" orb_status orbx_create(const orbx_config* cfg, orbx_handle** out) {
     ALLOC(h->d_depth, h->out_rows * sizeof(float));
     ALLOC(h->d_sad, h->out_rows * sizeof(int));
     ALLOC(h->d_pat, 256 * sizeof(uint32_t));
+    ALLOC(h->d_blur_frag, 256 * sizeof(uint32_t));
 #undef ALLOC
+    {
+        uint32_t frag[256];
+        orbdev::bm_fragments(frag);
+        if (cudaMemcpy(h->d_blur_frag, frag, sizeof(frag), cudaMemcpyHostToDevice) != cudaSuccess)
+            return fail(set_error(ORB_ERR_CUDA, "blur fragment upload failed"));
+    }
     {   // the rBRIEF pattern as 256 packed words (xa, ya, xb, yb), transposed to [pair % 8][pair / 8] for k_orient_describe
         static const int8_t pat[1024] = {
 #include "orb_pattern.inc"
@@ -410,7 +418,7 @@ extern "C" void orbx_destroy(orbx_handle* h) {
     orbr_release(h);
     void* ptrs[] = {h->d_pyr, h->d_blur, h->d_cand, h->d_sort, h->d_lvl_kp, h->d_slot, h->d_cand_cnt, h->d_lvl_cnt,
                     h->d_nkp, h->d_err, h->d_taps, h->d_kps, h->d_desc, h->d_node_scratch, h->d_stage, h->d_po,
-                    h->d_uright, h->d_depth, h->d_sad, h->d_cells, h->d_pat};
+                    h->d_uright, h->d_depth, h->d_sad, h->d_cells, h->d_pat, h->d_blur_frag};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (h->h_counts) cudaFreeHost(h->h_counts);
@@ -516,7 +524,18 @@ static orb_status run_pipeline(orbx_handle* h, int batch, int lap0, int lap1) {
     launch_p(k_offsets, dim3(1), dim3(32), 0, st, h->d_nkp, batch, h->d_offsets);
     ORB_LAUNCHED();
     if (prof) cudaEventRecord(h->ev[4], st);
-    if (h->blur_variant == 1) k_blur<true><<<dim3(g.totalTiles, batch), 256, 0, st>>>(g);    // horizontal pass by IDP.4A
+    if (h->blur_variant == 2) {   // both passes on the tensor cores (blur_mma.cuh), 128 x 96 tiles
+        BlurMmaPlan bp;
+        bp.frag = h->d_blur_frag;
+        int tiles = 0;
+        for (int l = 0; l < g.nlevels; ++l) {
+            bp.tileBase[l] = tiles;
+            bp.tilesX[l] = (g.lv[l].w + BM_TW - 1) / BM_TW;
+            tiles += bp.tilesX[l] * ((g.lv[l].h + BM_TH - 1) / BM_TH);
+        }
+        bp.tileBase[g.nlevels] = tiles;
+        ORB_CUDA(launch_blur_mma(g, bp, tiles, batch, st));
+    } else if (h->blur_variant == 1) k_blur<true><<<dim3(g.totalTiles, batch), 256, 0, st>>>(g);    // horizontal pass by IDP.4A
     else k_blur<false><<<dim3(g.totalTiles, batch), 256, 0, st>>>(g);
     ORB_LAUNCHED();
     if (prof) cudaEventRecord(h->ev[5], st);

@@ -18,7 +18,7 @@ struct orbx_handle {
     uint2* d_cells = nullptr;
     size_t cells_slots = 0;
     int fast_R = 0, fast_PW = 0, fast_LW = 0;
-    int blur_variant = 1;    // 1: k_blur<true> (IDP.4A horizontal pass, default), 0: k_blur<false>
+    int blur_variant = 2;    // 2: k_blur_mma (both passes as u8 IMMA, default), 1: k_blur<true> (IDP.4A horizontal pass), 0: k_blur<false>
     int resize_variant = 1;  // 1: k_resize_v2 (default), 0: k_resize
     bool fast_tma = false;   // ORB_FAST_TMA=1: k_fast_cells_v2<29, true> (window rows by cp.async.bulk + mbarrier)
     int qt_variant = 1;   // 1 (default): k_quadtree_v1; 0: k_quadtree (ORB_QT_VARIANT=0 at orbx_create)
@@ -53,6 +53,7 @@ struct orbx_handle {
     float* d_depth = nullptr;
     int* d_sad = nullptr;
     uint32_t* d_pat = nullptr;       // rBRIEF pattern, 256 packed pairs transposed for k_orient_describe
+    uint32_t* d_blur_frag = nullptr; // k_blur_mma: the lanes' constant A fragments (bm_fragments, 8 x 32 words)
     void* d_node_scratch = nullptr;
     uint8_t* d_stage = nullptr;
     uint8_t* d_po = nullptr;         // edge lists / results of orbo_pose_optimization_frames
