@@ -68,8 +68,22 @@ static void build_tables(orbx_handle* h) {
 // cv::resize INTER_LINEAR tap table: resize_core.cuh (shared with the host emulation of k_resize_v3)
 static void linear_taps(int ssize, int dsize, int2* out) { orbdev::rs_linear_taps(ssize, dsize, reinterpret_cast<int*>(out)); }
 
+// DistributeOctTree's sort element of a level (quadtree_core.cuh QtForm): the 64-bit, 12-depth form when a side of the region
+// (maxBorder - minBorder) exceeds 2048 px, the 32-bit, 11-depth form otherwise
+static bool qt_level_k64(const LevelGeom& L) {
+    return L.maxBX - 16 > orbdev::QtForm<uint32_t>::max_dim || L.maxBY - 16 > orbdev::QtForm<uint32_t>::max_dim;
+}
+
+// the region of level 0 (side - 32) must fit the 12-bit candidate coordinates and the 12-depth quadtree element
+static orb_status check_image_side(int w, int hh) {
+    const int lim = orbdev::QtForm<uint64_t>::max_dim + 32;
+    if (w > lim || hh > lim) return set_error(ORB_ERR_UNSUPPORTED, "image side > 4128 px is not supported (12-bit candidate coordinates)");
+    return ORB_OK;
+}
+
 // geometry for images of (w,h); (re)allocates nothing -- buffers are sized for max_width/max_height
 static orb_status plan_geometry(orbx_handle* h, int w, int hh) {
+    if (check_image_side(w, hh) != ORB_OK) return ORB_ERR_UNSUPPORTED;
     const int nl = h->cfg.n_levels;
     ExtractGeom& g = h->geom;
     memset(&g, 0, sizeof(g));
@@ -82,8 +96,6 @@ static orb_status plan_geometry(orbx_handle* h, int w, int hh) {
         LevelGeom& L = g.lv[l];
         L.w = (int)lrintf((float)w * h->inv_scale[l]);   // ORBextractor.cc:1691-1692
         L.h = (int)lrintf((float)hh * h->inv_scale[l]);
-        if (L.w > QT_MAX_DIM + 32 || L.h > QT_MAX_DIM + 32)
-            return set_error(ORB_ERR_UNSUPPORTED, "image side > 2080 px is not supported by the quadtree key");
         L.pitch = round_up(L.w, 16);
         L.blur_pitch = L.pitch;
         L.img_stride = (int64_t)L.pitch * L.h;
@@ -132,8 +144,8 @@ static orb_status plan_geometry(orbx_handle* h, int w, int hh) {
         L.kpCap = qt_node_cap(L.quota);   // the node list never exceeds N + 3 (quadtree_core.cuh)
         L.kpOff = kp;
         kp += L.kpCap;
-        L.sortOff = sortOff;
-        sortOff += pow2_ceil(L.candCap);
+        L.sortOff = sortOff;   // uint32 slots; every block is a power of two >= 4 slots, so 64-bit blocks stay 16-byte aligned
+        sortOff += pow2_ceil(L.candCap) * (qt_level_k64(L) ? 2 : 1);
         L.scale = h->scale[l];
         L.inv_scale = h->inv_scale[l];
         L.patch = (float)(int)(31 * h->scale[l]);   // ORBextractor.cc:1184
@@ -160,6 +172,7 @@ static orb_status plan_geometry(orbx_handle* h, int w, int hh) {
                     const int cw = std::min(x0 + L.wCell + 6, L.maxBX) - x0, ch = std::min(y0 + L.hCell + 6, L.maxBY) - y0;
                     if (cw < 7 || ch < 7) continue;
                     if (cw > 255 || ch > 255) return set_error(ORB_ERR_UNSUPPORTED, "FAST cell wider than 255 px");
+                    if (x0 > 0xfff || y0 > 0xfff) return set_error(ORB_ERR_UNSUPPORTED, "FAST cell origin beyond the 12-bit cell table");
                     h->cells_host.push_back(make_uint2((uint32_t)x0 | ((uint32_t)y0 << 12) | ((uint32_t)l << 24), (uint32_t)cw | ((uint32_t)ch << 8)));
                     const int tx0 = x0 + 3, tx1 = x0 + cw - 3;
                     const int gx0 = ((tx0 & ~3) - 4) & ~7, wd0 = ((tx0 & ~3) - gx0) >> 2, ngrp = ((tx1 - 1) >> 2) - (tx0 >> 2) + 1;
@@ -214,6 +227,7 @@ extern "C" int32_t orbx_max_features(const orbx_handle* h) {
 
 static orb_status apply_geometry(orbx_handle* h, int w, int hh) {
     if (w == h->cur_w && hh == h->cur_h) return ORB_OK;
+    if (check_image_side(w, hh) != ORB_OK) return ORB_ERR_UNSUPPORTED;   // before the handle's size: a refusal, not a usage error
     if (w > h->cfg.max_width || hh > h->cfg.max_height || w < 1 || hh < 1)
         return set_error(ORB_ERR_INVALID, "image larger than the handle's max_width/max_height");
     // pyramid base pointers are laid out for the CURRENT size inside the max-size allocation
@@ -265,9 +279,17 @@ static orb_status apply_geometry(orbx_handle* h, int w, int hh) {
     // per 37 tested pixels; provision area/24 and fall back to the global scratch beyond that.
     // Consecutive levels with the same capacity form a group (<= 4 groups, one launch each on its own stream).
     {
+        // Levels whose region side exceeds 2048 px (a prefix of the pyramid) sort 64-bit elements: they form one group of their own, run by
+        // k_quadtree_v1_k64; the other levels are grouped as before and keep their kernels.
         int capOf[ORB_MAX_LEVELS];
+        bool k64Of[ORB_MAX_LEVELS];
+        for (int l = 0; l < h->cfg.n_levels; ++l) k64Of[l] = qt_level_k64(h->geom.lv[l]);
+        if (k64Of[0] && (h->qt_variant == 0 || h->qt_max_groups == 4))
+            return set_error(ORB_ERR_UNSUPPORTED, "regions over 2048 px need k_quadtree_v1's 64-bit form: ORB_QT_VARIANT=0 and ORB_QT_GROUPS=4 "
+                                                  "support images up to 2080 px only");
         for (int l = 0; l < h->cfg.n_levels; ++l) {
             const LevelGeom& L = h->geom.lv[l];
+            const size_t esz = k64Of[l] ? 8 : 4;
             const int est = (int)((int64_t)(L.maxBX - 16) * (L.maxBY - 16) / 24);
             int c = pow2_ceil(std::max(est, 1024));
             c = std::min(c, 32768);
@@ -275,30 +297,37 @@ static orb_status apply_geometry(orbx_handle* h, int w, int hh) {
             else if (c > 4096 || (c > 2048 && h->qt_max_groups < 4)) c = 8192;
             else if (c > 2048) c = 4096;     // ORB_QT_GROUPS=4 only: levels 2-4 of a 640x480 pyramid sort <= 4096 keys
             else c = 2048;
-            while ((size_t)c * 4 + (h->qt_nodes_in_smem ? nodeBytes : 0) > 200 * 1024 && c > 2048) c >>= 1;
+            while ((size_t)c * esz + (h->qt_nodes_in_smem ? nodeBytes : 0) > 200 * 1024 && c > 2048) c >>= 1;
             capOf[l] = c;
         }
-        for (int l = 1; l < h->cfg.n_levels; ++l) capOf[l] = std::min(capOf[l], capOf[l - 1]);  // monotone
+        for (int l = 1; l < h->cfg.n_levels; ++l)
+            if (k64Of[l] == k64Of[l - 1]) capOf[l] = std::min(capOf[l], capOf[l - 1]);  // monotone within a form
+        const int k64Groups = k64Of[0] ? 1 : 0;
         h->qt_ngroups = 0;
         for (int l = 0; l < h->cfg.n_levels; ++l) {
-            if (h->qt_ngroups > 0 && (capOf[l] == h->qt_groups[h->qt_ngroups - 1].sort_cap || h->qt_ngroups == h->qt_max_groups)) {
+            const orbx_handle::QtGroup* P = h->qt_ngroups > 0 ? &h->qt_groups[h->qt_ngroups - 1] : nullptr;
+            if (P && P->k64 == k64Of[l] &&
+                (k64Of[l] || capOf[l] == P->sort_cap || h->qt_ngroups - k64Groups == h->qt_max_groups)) {
                 h->qt_groups[h->qt_ngroups - 1].level_end = l + 1;
             } else {
                 orbx_handle::QtGroup& G = h->qt_groups[h->qt_ngroups++];
                 G.level_begin = l;
                 G.level_end = l + 1;
                 G.sort_cap = capOf[l];
+                G.k64 = k64Of[l];
             }
         }
-        size_t maxSmem = 0;
+        size_t maxSmem = 0, maxSmem64 = 0;
         for (int i = 0; i < h->qt_ngroups; ++i) {
             // a group that absorbed smaller levels keeps its (larger) capacity: always sufficient
-            h->qt_groups[i].smem = (size_t)h->qt_groups[i].sort_cap * 4 + (h->qt_nodes_in_smem ? nodeBytes : 0);
-            maxSmem = std::max(maxSmem, h->qt_groups[i].smem);
+            orbx_handle::QtGroup& G = h->qt_groups[i];
+            G.smem = (size_t)G.sort_cap * (G.k64 ? 8 : 4) + (h->qt_nodes_in_smem ? nodeBytes : 0);
+            (G.k64 ? maxSmem64 : maxSmem) = std::max(G.k64 ? maxSmem64 : maxSmem, G.smem);
         }
         ORB_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxSmem));
         ORB_CUDA(cudaFuncSetAttribute(k_quadtree_v1<QT_THREADS, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxSmem));
         ORB_CUDA(cudaFuncSetAttribute(k_quadtree_v1<1024, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxSmem));
+        if (k64Groups) ORB_CUDA(qt_k64_set_smem(maxSmem64));   // quadtree_k64.cu (liborbslam3_b200_qt64.so)
     }
     const size_t ordBytes = ((size_t)h->geom.kpTotal + 64) * 4;
     ORB_CUDA(cudaFuncSetAttribute(k_order, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(ordBytes, (size_t)1024)));
@@ -508,11 +537,18 @@ static orb_status run_pipeline(orbx_handle* h, int batch, int lap0, int lap1) {
         const orbx_handle::QtGroup& Q = h->qt_groups[gi];
         cudaStream_t qs = gi == 0 ? st : h->aux_stream[gi - 1];
         if (gi > 0) cudaStreamWaitEvent(qs, h->ev_fork, 0);
-        const bool wide = h->qt_variant == 1 && Q.level_begin == 0;      // the group with level 0: 1024 threads per CTA
-        launch_p(h->qt_variant == 0 ? k_quadtree : wide ? k_quadtree_v1<1024, 1> : k_quadtree_v1<QT_THREADS, 4>,
-                 dim3(batch * (Q.level_end - Q.level_begin)), dim3(wide ? 1024 : QT_THREADS), Q.smem, qs,
-                 g, batch, Q.level_begin, h->d_cand, h->d_cand_cnt, h->d_sort, (char*)h->d_node_scratch,
-                 (int64_t)h->qt_node_stride, Q.sort_cap, h->qt_nodes_in_smem, h->qt_node_cap, h->d_lvl_kp, h->d_lvl_cnt, h->d_err);
+        // 1024 threads per CTA for the group with level 0 and, after a 64-bit group, for the first 32-bit group (the largest levels of
+        // each form).  The 64-bit group always holds level 0.
+        const bool wide = h->qt_variant == 1 && (gi == 0 || (gi == 1 && h->qt_groups[0].k64));
+        if (Q.k64)   // k_quadtree_v1_k64 lives in liborbslam3_b200_qt64.so: its launch error comes back from there
+            ORB_CUDA(launch_quadtree_k64(batch * (Q.level_end - Q.level_begin), Q.smem, qs, g, batch, Q.level_begin, h->d_cand, h->d_cand_cnt,
+                                         h->d_sort, (char*)h->d_node_scratch, (int64_t)h->qt_node_stride, Q.sort_cap, h->qt_nodes_in_smem,
+                                         h->qt_node_cap, h->d_lvl_kp, h->d_lvl_cnt, h->d_err));
+        else
+            launch_p(h->qt_variant == 0 ? k_quadtree : wide ? k_quadtree_v1<1024, 1> : k_quadtree_v1<QT_THREADS, 4>,
+                     dim3(batch * (Q.level_end - Q.level_begin)), dim3(wide ? 1024 : QT_THREADS), Q.smem, qs,
+                     g, batch, Q.level_begin, h->d_cand, h->d_cand_cnt, h->d_sort, (char*)h->d_node_scratch,
+                     (int64_t)h->qt_node_stride, Q.sort_cap, h->qt_nodes_in_smem, h->qt_node_cap, h->d_lvl_kp, h->d_lvl_cnt, h->d_err);
         ORB_LAUNCHED();
         if (gi > 0) {
             cudaEventRecord(h->ev_join[gi - 1], qs);

@@ -68,7 +68,7 @@ struct orbx_handle {
     int last_batch = 0;
     // quadtree launch plan: up to 4 level groups with their own shared-memory size, run on parallel
     // streams (forked from / joined into `stream`)
-    struct QtGroup { int level_begin, level_end, sort_cap; size_t smem; };
+    struct QtGroup { int level_begin, level_end, sort_cap; size_t smem; bool k64; };   // k64: k_quadtree_v1_k64 (regions over 2048 px)
     QtGroup qt_groups[4] = {};
     int qt_max_groups = 3;   // level groups (launches) of the quadtree stage: {16384+, 8192, 2048} sort capacities; ORB_QT_GROUPS=4 adds a 4096 group
                              // (measured in round 2: 16 KB less shared memory for levels 2-4, but 0.317 instead of 0.278 ms per batch -- more

@@ -5,6 +5,7 @@
 #include "common.cuh"
 #include "devmath.cuh"
 #include "quadtree_core.cuh"
+#include "quadtree_v1.cuh"
 #include "resize_core.cuh"
 
 namespace orb {
@@ -430,67 +431,11 @@ __global__ void __launch_bounds__(QT_THREADS) k_quadtree(const __grid_constant__
 // instead of run by thread 0 (both in quadtree_sort_par.cuh).  A separate
 // kernel so that k_quadtree -- green on the GPU tier -- keeps its machine code bit for bit (scripts/sass_fingerprint.py);
 // selected with ORB_QT_VARIANT=1 at orbx_create until it has had its own device run.
-__device__ __forceinline__ int qt_run_v1(uint32_t* arr, void* ws, int cap, int n, int npow, const uint32_t* __restrict__ src,
-                                         const QtGeom& q, uint32_t* out) {
-    QT_PROF_BEGIN();
-    if (npow < 256) npow = 256;     // qt_bitonic_sort_w sorts whole 256-element warp blocks (every sort buffer holds >= 2048 elements)
-    for (int i = threadIdx.x; i < npow; i += blockDim.x) arr[i] = (i < n) ? qt_element(src[i], q) : 0xffffffffu;
-    __syncthreads();
-    QT_TICK(q, 0)
-    qt_bitonic_sort_w(arr, npow);
-    QT_TICK(q, 1)
-    QtWork w;
-    qt_work_carve(w, ws, cap);
-    return qt_distribute_v<1>(arr, n, q, w, out);
-}
-
 // MAXT = 256 (four CTAs per SM) for the small levels; MAXT = 1024 for the group that holds level 0, whose 128-per-batch CTAs each sort
 // 4-8 k candidates: one CTA per SM either way, so four times the threads shorten the longest kernel of the stage.  The body only uses
 // blockDim.x (QT_PAR_FOR, qt_exscan), never QT_THREADS.
 template <int MAXT, int MINB>
-__global__ void __launch_bounds__(MAXT, MINB) k_quadtree_v1(const __grid_constant__ ExtractGeom g, int batch, int levelBegin,
-                                                           const uint32_t* __restrict__ cand, const int* __restrict__ candCnt,
-                                                           uint32_t* __restrict__ sortScratch, char* __restrict__ nodeScratch,
-                                                           int64_t nodeScratchStride, int sortCapSmem, int nodesInSmem,
-                                                           int nodeCapMax, uint32_t* __restrict__ lvlKp, int* __restrict__ lvlCnt,
-                                                           int* __restrict__ err) {
-    extern __shared__ __align__(16) unsigned char qt_smem[];
-    const int l = levelBegin + blockIdx.x / batch, img = blockIdx.x % batch;
-    const LevelGeom& G = g.lv[l];
-    int n = candCnt[img * g.nlevels + l];
-    if (n > G.candCap) n = G.candCap;
-    QtGeom q;
-    q.regionW = G.maxBX - 16; q.regionH = G.maxBY - 16;
-    q.nIni = G.nIni; q.hX = G.hX; q.N = G.quota;
-    q.wCell = G.wCell; q.hCell = G.hCell; q.nCols = G.nCols;
-#if defined(QT_PROFILE)
-    q.prof_base = l == 0 ? 0 : 16;
-#endif
-    int npow = 2;
-    while (npow < n) npow <<= 1;
-    const uint32_t* src = cand + (int64_t)img * g.candTotal + G.candOff;
-    uint32_t* out = lvlKp + (int64_t)img * g.kpTotal + G.kpOff;
-    int cap = qt_node_cap(G.quota);
-    if (cap > nodeCapMax) cap = nodeCapMax;
-    uint32_t* garr = sortScratch + (int64_t)img * g.sortTotal + G.sortOff;
-    void* gws = nodeScratch + ((int64_t)l * batch + img) * nodeScratchStride;
-    int S;
-    if (npow <= sortCapSmem) {
-        uint32_t* sarr = reinterpret_cast<uint32_t*>(qt_smem);
-        if (nodesInSmem) S = qt_run_v1(sarr, qt_smem + (size_t)sortCapSmem * 4, cap, n, npow, src, q, out);
-        else S = qt_run_v1(sarr, gws, cap, n, npow, src, q, out);
-    } else {
-        if (nodesInSmem) S = qt_run_v1(garr, qt_smem + (size_t)sortCapSmem * 4, cap, n, npow, src, q, out);
-        else S = qt_run_v1(garr, gws, cap, n, npow, src, q, out);
-    }
-    if (threadIdx.x == 0) {
-        if (S < 0 || S > G.kpCap) {
-            atomicExch(&err[1], 1);
-            S = 0;
-        }
-        lvlCnt[img * g.nlevels + l] = S;
-    }
-}
+__global__ void __launch_bounds__(MAXT, MINB) k_quadtree_v1(QT_V1_PARAMS) { qt_v1_body<uint32_t>(QT_V1_ARGS); }
 
 // ---------------------------------------------------------------------------------------------
 // K3b  output slot of every keypoint (ORBextractor.cc:1656-1678): emission order is level-major;

@@ -3,7 +3,8 @@
 //
 // The reference walks a std::list of nodes that each own a copy of their keypoints.  Here:
 //   * every candidate computes its own root-to-leaf path (it depends only on its coordinates) and is
-//     packed into ONE 32-bit word  [root:2 | path:22 (2 bits/depth, 11 depths) | score:8];
+//     packed into ONE sort element [root:2 | path:2 bits/depth | score:8] (QtForm below: 32 bits and 11
+//     depths for regions up to 2048 px, 64 bits and 12 depths up to 4096 px);
 //   * the words are sorted (bitonic, in shared memory), after which every tree node is a contiguous
 //     range and "DivideNode" is three binary searches -- no keypoint is ever moved again;
 //   * the node list is an array rebuilt per round with prefix sums (the list order, push_front
@@ -23,8 +24,15 @@
 
 namespace orbdev {
 
-#define QT_LEVELS 11               // path depths stored per candidate (region side <= 2048 px)
-#define QT_MAX_DIM 2048
+// The two forms of the sort element; the algorithm below is written once and instantiated for both.  A region of side
+// 2^depths px is one pixel wide after `depths` halvings, so the path identifies the candidate's pixel.
+//   uint32_t: [root:2 | path:22 | score:8]                  regions up to 2048 px (k_quadtree, k_quadtree_v1)
+//   uint64_t: [0:30 | root:2 | path:24 | score:8]           regions up to 4096 px (k_quadtree_v1_k64)
+// QtNode::pd holds depth << pd_shift | prefix; the prefix of a depth-d node has 2 + 2d bits.
+template <typename E> struct QtForm;
+template <> struct QtForm<uint32_t> { static constexpr int depths = 11, max_dim = 2048, pd_shift = 24; };
+template <> struct QtForm<uint64_t> { static constexpr int depths = 12, max_dim = 4096, pd_shift = 28; };
+template <typename E> ORB_HD constexpr int qt_elem_bits() { return 10 + 2 * QtForm<E>::depths; }
 
 #if defined(__CUDA_ARCH__)
 #define QT_PAR_FOR(i, n) for (int i = threadIdx.x; i < (n); i += blockDim.x)
@@ -69,7 +77,7 @@ __device__ long long g_qt_prof[32];
 
 struct QtNode {      // 20 bytes
     int lo, hi;      // candidate range [lo,hi) in the sorted array
-    uint32_t pd;     // depth << 24 | prefix (root + 2*depth path bits)
+    uint32_t pd;     // depth << QtForm::pd_shift | prefix (root + 2*depth path bits)
     int16_t ulx, uly, urx, bry;
 };
 
@@ -128,34 +136,38 @@ ORB_HD void qt_work_carve(QtWork& w, void* base, int cap) {
 ORB_HD uint32_t qt_pack_cand(int x, int y, int score) { return (uint32_t)x | ((uint32_t)y << 12) | ((uint32_t)score << 24); }
 
 // sortable element of a candidate
-ORB_HD uint32_t qt_element(uint32_t cand, const QtGeom& g) {
+template <typename E = uint32_t>
+ORB_HD E qt_element(uint32_t cand, const QtGeom& g) {
     const int x = cand & 0xfff, y = (cand >> 12) & 0xfff;
     const int root = (int)fdiv((float)x, g.hX);
     QtBox b = qt_root_box(root, g.hX, g.regionH);
-    uint32_t key = (uint32_t)root;
-    for (int d = 0; d < QT_LEVELS; ++d) {
+    E key = (E)root;
+    for (int d = 0; d < QtForm<E>::depths; ++d) {
         const int mx = b.ulx + ((b.urx - b.ulx + 1) >> 1);
         const int my = b.uly + ((b.bry - b.uly + 1) >> 1);
         const int q = (x < mx ? 0 : 1) | (y < my ? 0 : 2);
-        key = (key << 2) | (uint32_t)q;
+        key = (key << 2) | (E)q;
         b = qt_child_box(b, q);
     }
-    return (key << 8) | (cand >> 24);
+    return (key << 8) | (E)(cand >> 24);
 }
 
-// recover (x_rel, y_rel) of an element by replaying its path: after QT_LEVELS halvings the box is
+// recover (x_rel, y_rel) of an element by replaying its path: after QtForm<E>::depths halvings the box is
 // at most one pixel wide, so its upper-left corner is the point.
-ORB_HD void qt_element_xy(uint32_t e, const QtGeom& g, int* x, int* y) {
-    const int root = (int)(e >> 30);
+template <typename E>
+ORB_HD void qt_element_xy(E e, const QtGeom& g, int* x, int* y) {
+    const int root = (int)(e >> (qt_elem_bits<E>() - 2));
     QtBox b = qt_root_box(root, g.hX, g.regionH);
-    for (int d = 0; d < QT_LEVELS; ++d) b = qt_child_box(b, (int)((e >> (28 - 2 * d)) & 3u));
+    for (int d = 0; d < QtForm<E>::depths; ++d) b = qt_child_box(b, (int)((e >> (qt_elem_bits<E>() - 4 - 2 * d)) & 3u));
     *x = b.ulx;
     *y = b.uly;
 }
 
-ORB_HD int qt_node_shift(int depth) { return 30 - 2 * depth; }
+template <typename E = uint32_t>
+ORB_HD int qt_node_shift(int depth) { return qt_elem_bits<E>() - 2 - 2 * depth; }
 
-ORB_HD int qt_lower_bound(const uint32_t* a, int lo, int hi, uint32_t v) {
+template <typename E>
+ORB_HD int qt_lower_bound(const E* a, int lo, int hi, E v) {
     while (lo < hi) {
         const int mid = (lo + hi) >> 1;
         if (a[mid] < v) lo = mid + 1; else hi = mid;
@@ -281,13 +293,14 @@ inline void qt_exscan3(int* a, int* b, int* c, int n, int* tmp, int* ta, int* tb
 #endif
 
 // bitonic sort of arr[0..npow) (npow a power of two), ascending
-ORB_HD void qt_bitonic_sort(uint32_t* arr, int npow) {
+template <typename E>
+ORB_HD void qt_bitonic_sort(E* arr, int npow) {
     for (int k = 2; k <= npow; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
             QT_PAR_FOR(i, npow >> 1) {
                 const int l = ((i & ~(j - 1)) << 1) | (i & (j - 1));
                 const int r = l | j;
-                const uint32_t a = arr[l], b = arr[r];
+                const E a = arr[l], b = arr[r];
                 const bool up = (l & k) == 0;
                 if ((a > b) == up) {
                     arr[l] = b;
@@ -300,13 +313,14 @@ ORB_HD void qt_bitonic_sort(uint32_t* arr, int npow) {
 }
 
 // children of node `nd`: boundaries b[0..2] (b0=lo, b4=hi implicit) -> counts; returns m | x << 8
-ORB_HD int qt_split(const uint32_t* arr, const QtNode& nd, int* b3) {
-    const int depth = (int)(nd.pd >> 24);
-    const uint32_t pref = nd.pd & 0xffffffu;
-    const int sh = qt_node_shift(depth + 1);
+template <typename E>
+ORB_HD int qt_split(const E* arr, const QtNode& nd, int* b3) {
+    const int depth = (int)(nd.pd >> QtForm<E>::pd_shift);
+    const uint32_t pref = nd.pd & ((1u << QtForm<E>::pd_shift) - 1u);
+    const int sh = qt_node_shift<E>(depth + 1);
     int prev = nd.lo, m = 0, x = 0;
     for (int q = 1; q <= 4; ++q) {
-        const int b = (q < 4) ? qt_lower_bound(arr, prev, nd.hi, ((pref << 2) | (uint32_t)q) << sh) : nd.hi;
+        const int b = (q < 4) ? qt_lower_bound(arr, prev, nd.hi, (E)((pref << 2) | (uint32_t)q) << sh) : nd.hi;
         if (q < 4) b3[q - 1] = b;
         const int c = b - prev;
         m += c > 0;
@@ -316,21 +330,23 @@ ORB_HD int qt_split(const uint32_t* arr, const QtNode& nd, int* b3) {
     return m | (x << 8);
 }
 
+template <typename E>
 ORB_HD QtNode qt_child(const QtNode& nd, const int* b3, int q) {
-    const int depth = (int)(nd.pd >> 24);
-    const uint32_t pref = nd.pd & 0xffffffu;
+    const int depth = (int)(nd.pd >> QtForm<E>::pd_shift);
+    const uint32_t pref = nd.pd & ((1u << QtForm<E>::pd_shift) - 1u);
     QtBox pb;
     pb.ulx = nd.ulx; pb.uly = nd.uly; pb.urx = nd.urx; pb.bry = nd.bry;
     const QtBox cb = qt_child_box(pb, q);
     QtNode c;
     c.lo = q == 0 ? nd.lo : b3[q - 1];
     c.hi = q == 3 ? nd.hi : b3[q];
-    c.pd = ((uint32_t)(depth + 1) << 24) | ((pref << 2) | (uint32_t)q);
+    c.pd = ((uint32_t)(depth + 1) << QtForm<E>::pd_shift) | ((pref << 2) | (uint32_t)q);
     c.ulx = (int16_t)cb.ulx; c.uly = (int16_t)cb.uly; c.urx = (int16_t)cb.urx; c.bry = (int16_t)cb.bry;
     return c;
 }
 
-ORB_HD bool qt_expandable(const QtNode& nd) { return (nd.hi - nd.lo) > 1 && (int)(nd.pd >> 24) < QT_LEVELS; }
+template <typename E>
+ORB_HD bool qt_expandable(const QtNode& nd) { return (nd.hi - nd.lo) > 1 && (int)(nd.pd >> QtForm<E>::pd_shift) < QtForm<E>::depths; }
 
 // compareNodes (ORBextractor.cc:676-697) orders by (point count, UL.x): one 48-bit key, compared without branches
 ORB_HD uint64_t qt_item_key(const QtItem& a) { return ((uint64_t)a.cnt << 16) | (uint64_t)(a.ulx_pos >> 16); }
@@ -471,15 +487,15 @@ ORB_HD uint64_t qt_order_key(int x, int y, const QtGeom& g) {
 // ---------------------------------------------------------------------------------------------
 // VARIANT 0: the ordered phase's std::sort by one thread (GPU-validated in round 1).  VARIANT 1: the same moves spread over the
 // CTA (quadtree_sort_par.cuh; host-emulated in tests/test_quadtree_emul.py; the default since its round-2 device run).
-template <int VARIANT>
-ORB_HD int qt_distribute_v(const uint32_t* arr, int n, const QtGeom& g, QtWork& w, uint32_t* out) {
+template <int VARIANT, typename Key>
+ORB_HD int qt_distribute_v(const Key* arr, int n, const QtGeom& g, QtWork& w, uint32_t* out) {
     // roots (ORBextractor.cc:718-786): non-empty ones, in order
     QT_PROF_BEGIN();
     int S = 0;
     QT_SERIAL {
         int lo = 0, cnt = 0;
         for (int r = 0; r < g.nIni; ++r) {
-            const int hi = (r == 3) ? n : qt_lower_bound(arr, lo, n, (uint32_t)(r + 1) << 30);
+            const int hi = (r == 3) ? n : qt_lower_bound(arr, lo, n, (Key)(r + 1) << (qt_elem_bits<Key>() - 2));
             if (hi > lo) {
                 QtNode nd;
                 const QtBox b = qt_root_box(r, g.hX, g.regionH);
@@ -502,7 +518,7 @@ ORB_HD int qt_distribute_v(const uint32_t* arr, int n, const QtGeom& g, QtWork& 
         // ---- one sweep over the list (ORBextractor.cc:814-906) --------------------------------
         QT_PAR_FOR(t, S) {
             const QtNode nd = w.cur[t];
-            if (qt_expandable(nd)) {
+            if (qt_expandable<Key>(nd)) {
                 const int mx = qt_split(arr, nd, &w.bnd[3 * t]);
                 w.m[t] = mx & 0xff;
                 w.x[t] = mx >> 8;
@@ -520,7 +536,7 @@ ORB_HD int qt_distribute_v(const uint32_t* arr, int n, const QtGeom& g, QtWork& 
         if (E + NM > w.cap) return -1;
         QT_PAR_FOR(t, S) {
             const QtNode nd = w.cur[t];
-            if (!qt_expandable(nd)) {
+            if (!qt_expandable<Key>(nd)) {
                 w.nxt[E + w.f[t]] = nd;
             } else {
                 const int* b3 = &w.bnd[3 * t];
@@ -534,7 +550,7 @@ ORB_HD int qt_distribute_v(const uint32_t* arr, int n, const QtGeom& g, QtWork& 
                 for (int q = 3; q >= 0; --q)
                     if (cnts[q] > 0) {
                         pos[q] = base + r;
-                        w.nxt[base + r] = qt_child(nd, b3, q);
+                        w.nxt[base + r] = qt_child<Key>(nd, b3, q);
                         ++r;
                     }
                 int rr = 0;
@@ -646,7 +662,7 @@ ORB_HD int qt_distribute_v(const uint32_t* arr, int n, const QtGeom& g, QtWork& 
                     for (int q = 3; q >= 0; --q)
                         if (cnts[q] > 0) {
                             pos[q] = base + r;
-                            w.nxt[base + r] = qt_child(nd, b3, q);
+                            w.nxt[base + r] = qt_child<Key>(nd, b3, q);
                             ++r;
                         }
                     int rr = 0;
@@ -673,13 +689,13 @@ ORB_HD int qt_distribute_v(const uint32_t* arr, int n, const QtGeom& g, QtWork& 
     // ---- best candidate of every leaf (ORBextractor.cc:1028-1053) ------------------------------
     QT_PAR_FOR(t, S) {
         const QtNode nd = w.cur[t];
-        uint32_t best = arr[nd.lo];
+        Key best = arr[nd.lo];
         int bx, by;
         qt_element_xy(best, g, &bx, &by);
         uint64_t bkey = qt_order_key(bx, by, g);
         for (int i = nd.lo + 1; i < nd.hi; ++i) {
-            const uint32_t e = arr[i];
-            const uint32_t se = e & 0xffu, sb = best & 0xffu;
+            const Key e = arr[i];
+            const uint32_t se = (uint32_t)e & 0xffu, sb = (uint32_t)best & 0xffu;
             if (se < sb) continue;
             int ex, ey;
             qt_element_xy(e, g, &ex, &ey);
@@ -688,14 +704,15 @@ ORB_HD int qt_distribute_v(const uint32_t* arr, int n, const QtGeom& g, QtWork& 
                 best = e; bx = ex; by = ey; bkey = ekey;
             }
         }
-        out[t] = qt_pack_cand(bx, by, (int)(best & 0xffu));
+        out[t] = qt_pack_cand(bx, by, (int)((uint32_t)best & 0xffu));
     }
     QT_SYNC();
     QT_TICK(g, 7)
     return S;
 }
 
-ORB_HD int qt_distribute(const uint32_t* arr, int n, const QtGeom& g, QtWork& w, uint32_t* out) {
+template <typename E>
+ORB_HD int qt_distribute(const E* arr, int n, const QtGeom& g, QtWork& w, uint32_t* out) {
     return qt_distribute_v<0>(arr, n, g, w, out);
 }
 

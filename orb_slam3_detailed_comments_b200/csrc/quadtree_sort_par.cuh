@@ -332,16 +332,17 @@ ORB_HD void qt_std_sort_items_par(QtItem* a, int n, QtItem* tmp, int* seg, int* 
 // levels in registers and stores them -- half the barriers and half the shared-memory round trips of qt_bitonic_sort; an odd
 // stage count leaves one ordinary pass (j = 1).  Keys are unique per candidate pixel (root | path | score), so any correct sort
 // yields the same array.
-ORB_HD void qt_bitonic_sort_r4(uint32_t* arr, int npow) {
+template <typename E>
+ORB_HD void qt_bitonic_sort_r4(E* arr, int npow) {
     for (int k = 2; k <= npow; k <<= 1) {
         int j = k >> 1;
         for (; j >= 2; j >>= 2) {
             const int h = j >> 1;
             QT_PAR_FOR(i, npow >> 2) {
                 const int l0 = (i & (h - 1)) | ((i & ~(h - 1)) << 2);   // i spread over the index bits other than h and j = 2h
-                uint32_t a0 = arr[l0], a1 = arr[l0 | h], a2 = arr[l0 | j], a3 = arr[l0 | j | h];
+                E a0 = arr[l0], a1 = arr[l0 | h], a2 = arr[l0 | j], a3 = arr[l0 | j | h];
                 const bool up = (l0 & k) == 0;
-                uint32_t x;
+                E x;
                 if ((a0 > a2) == up) { x = a0; a0 = a2; a2 = x; }
                 if ((a1 > a3) == up) { x = a1; a1 = a3; a3 = x; }
                 if ((a0 > a1) == up) { x = a0; a0 = a1; a1 = x; }
@@ -353,7 +354,7 @@ ORB_HD void qt_bitonic_sort_r4(uint32_t* arr, int npow) {
         if (j == 1) {
             QT_PAR_FOR(i, npow >> 1) {
                 const int l = i << 1, r = l | 1;
-                const uint32_t a = arr[l], b = arr[r];
+                const E a = arr[l], b = arr[r];
                 if ((a > b) == ((l & k) == 0)) { arr[l] = b; arr[r] = a; }
             }
             QT_SYNC();
@@ -364,16 +365,17 @@ ORB_HD void qt_bitonic_sort_r4(uint32_t* arr, int npow) {
 // The same with up to THREE butterfly stages per pass (strides j, j/2, j/4: eight elements per thread, twelve compare-exchanges in
 // registers); a remainder of two stages takes the four-element step, of one the ordinary pass.  8192 elements: 35 barriers instead
 // of 49 (91 for one stage per pass).
-ORB_HD void qt_bitonic_sort_r8(uint32_t* arr, int npow) {
-#define QT_CX(x, y) { if (((x) > (y)) == up) { const uint32_t t_ = (x); (x) = (y); (y) = t_; } }
+template <typename E>
+ORB_HD void qt_bitonic_sort_r8(E* arr, int npow) {
+#define QT_CX(x, y) { if (((x) > (y)) == up) { const E t_ = (x); (x) = (y); (y) = t_; } }
     for (int k = 2; k <= npow; k <<= 1) {
         int j = k >> 1;
         for (; j >= 4; j >>= 3) {
             const int h = j >> 1, q = j >> 2;
             QT_PAR_FOR(i, npow >> 3) {
                 const int l0 = (i & (q - 1)) | ((i & ~(q - 1)) << 3);   // i spread over the index bits other than q, h = 2q, j = 4q
-                uint32_t a0 = arr[l0], a1 = arr[l0 | q], a2 = arr[l0 | h], a3 = arr[l0 | h | q];
-                uint32_t a4 = arr[l0 | j], a5 = arr[l0 | j | q], a6 = arr[l0 | j | h], a7 = arr[l0 | j | h | q];
+                E a0 = arr[l0], a1 = arr[l0 | q], a2 = arr[l0 | h], a3 = arr[l0 | h | q];
+                E a4 = arr[l0 | j], a5 = arr[l0 | j | q], a6 = arr[l0 | j | h], a7 = arr[l0 | j | h | q];
                 const bool up = (l0 & k) == 0;
                 QT_CX(a0, a4) QT_CX(a1, a5) QT_CX(a2, a6) QT_CX(a3, a7)        // stride j
                 QT_CX(a0, a2) QT_CX(a1, a3) QT_CX(a4, a6) QT_CX(a5, a7)        // stride h
@@ -386,7 +388,7 @@ ORB_HD void qt_bitonic_sort_r8(uint32_t* arr, int npow) {
         if (j == 2) {          // two stages left: strides 2 and 1
             QT_PAR_FOR(i, npow >> 2) {
                 const int l0 = i << 2;
-                uint32_t a0 = arr[l0], a1 = arr[l0 | 1], a2 = arr[l0 | 2], a3 = arr[l0 | 3];
+                E a0 = arr[l0], a1 = arr[l0 | 1], a2 = arr[l0 | 2], a3 = arr[l0 | 3];
                 const bool up = (l0 & k) == 0;
                 QT_CX(a0, a2) QT_CX(a1, a3) QT_CX(a0, a1) QT_CX(a2, a3)
                 arr[l0] = a0; arr[l0 | 1] = a1; arr[l0 | 2] = a2; arr[l0 | 3] = a3;
@@ -395,7 +397,7 @@ ORB_HD void qt_bitonic_sort_r8(uint32_t* arr, int npow) {
         } else if (j == 1) {   // one stage left
             QT_PAR_FOR(i, npow >> 1) {
                 const int l = i << 1;
-                uint32_t a0 = arr[l], a1 = arr[l | 1];
+                E a0 = arr[l], a1 = arr[l | 1];
                 const bool up = (l & k) == 0;
                 QT_CX(a0, a1)
                 arr[l] = a0; arr[l | 1] = a1;
@@ -416,9 +418,10 @@ ORB_HD void qt_bitonic_sort_r8(uint32_t* arr, int npow) {
 // up to 256 run in one such pass; a larger merge takes shared-memory passes (three / two / one stage each, strides >= 256 only:
 // conflict-free) followed by one warp pass.  8192 elements: 13 barriers (35 before, 91 with one stage per pass).  Keys are unique,
 // so any correct sort gives the same array.
-__device__ __forceinline__ void qt_warp_stages(uint32_t (&v)[8], int idx0, int k, int jstart, int lane) {
+template <typename E>
+__device__ __forceinline__ void qt_warp_stages(E (&v)[8], int idx0, int k, int jstart, int lane) {
 #define QT_IDX(e) (idx0 + ((e) & 3) + (((e) >> 2) << 7))
-#define QT_CXU(x, y, up) { const uint32_t lo_ = min((x), (y)), hi_ = max((x), (y)); (x) = (up) ? lo_ : hi_; (y) = (up) ? hi_ : lo_; }
+#define QT_CXU(x, y, up) { const E lo_ = min((x), (y)), hi_ = max((x), (y)); (x) = (up) ? lo_ : hi_; (y) = (up) ? hi_ : lo_; }
 #pragma unroll
     for (int s = 7; s >= 0; --s) {
         const int j = 1 << s;
@@ -432,7 +435,7 @@ __device__ __forceinline__ void qt_warp_stages(uint32_t (&v)[8], int idx0, int k
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
                 const bool up = (QT_IDX(e) & k) == 0;
-                const uint32_t other = __shfl_xor_sync(0xffffffffu, v[e], m);
+                const E other = __shfl_xor_sync(0xffffffffu, v[e], m);
                 v[e] = (lower == up) ? min(v[e], other) : max(v[e], other);
             }
         } else if (s == 1) {
@@ -447,10 +450,12 @@ __device__ __forceinline__ void qt_warp_stages(uint32_t (&v)[8], int idx0, int k
 #undef QT_CXU
 }
 
-// npow: a power of two >= 256; arr 16-byte aligned; whole CTA (blockDim a multiple of 32); returns after a barrier
-__device__ inline void qt_bitonic_sort_w(uint32_t* arr, int npow) {
+// npow: a power of two >= 256; arr 16-byte aligned; whole CTA (blockDim a multiple of 32); returns after a barrier.  E = uint64_t (the
+// 12-depth form): a lane's four consecutive elements are two 16-byte accesses instead of one.
+template <typename E>
+__device__ inline void qt_bitonic_sort_w(E* arr, int npow) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5, nblk = npow >> 8;
-#define QT_CX(x, y) { if (((x) > (y)) == up) { const uint32_t t_ = (x); (x) = (y); (y) = t_; } }
+#define QT_CX(x, y) { if (((x) > (y)) == up) { const E t_ = (x); (x) = (y); (y) = t_; } }
     for (int kk = 256; kk <= npow; kk <<= 1) {
         // shared-memory passes for the strides >= 256 of merge size kk (none for kk == 256)
         int j = kk >> 1;
@@ -458,8 +463,8 @@ __device__ inline void qt_bitonic_sort_w(uint32_t* arr, int npow) {
             const int h = j >> 1, q = j >> 2;
             for (int i = threadIdx.x; i < (npow >> 3); i += blockDim.x) {
                 const int l0 = (i & (q - 1)) | ((i & ~(q - 1)) << 3);
-                uint32_t a0 = arr[l0], a1 = arr[l0 | q], a2 = arr[l0 | h], a3 = arr[l0 | h | q];
-                uint32_t a4 = arr[l0 | j], a5 = arr[l0 | j | q], a6 = arr[l0 | j | h], a7 = arr[l0 | j | h | q];
+                E a0 = arr[l0], a1 = arr[l0 | q], a2 = arr[l0 | h], a3 = arr[l0 | h | q];
+                E a4 = arr[l0 | j], a5 = arr[l0 | j | q], a6 = arr[l0 | j | h], a7 = arr[l0 | j | h | q];
                 const bool up = (l0 & kk) == 0;
                 QT_CX(a0, a4) QT_CX(a1, a5) QT_CX(a2, a6) QT_CX(a3, a7)
                 QT_CX(a0, a2) QT_CX(a1, a3) QT_CX(a4, a6) QT_CX(a5, a7)
@@ -472,7 +477,7 @@ __device__ inline void qt_bitonic_sort_w(uint32_t* arr, int npow) {
         if (j == 512) {          // strides 512 and 256
             for (int i = threadIdx.x; i < (npow >> 2); i += blockDim.x) {
                 const int l0 = (i & 255) | ((i & ~255) << 2);
-                uint32_t a0 = arr[l0], a1 = arr[l0 | 256], a2 = arr[l0 | 512], a3 = arr[l0 | 768];
+                E a0 = arr[l0], a1 = arr[l0 | 256], a2 = arr[l0 | 512], a3 = arr[l0 | 768];
                 const bool up = (l0 & kk) == 0;
                 QT_CX(a0, a2) QT_CX(a1, a3) QT_CX(a0, a1) QT_CX(a2, a3)
                 arr[l0] = a0; arr[l0 | 256] = a1; arr[l0 | 512] = a2; arr[l0 | 768] = a3;
@@ -481,7 +486,7 @@ __device__ inline void qt_bitonic_sort_w(uint32_t* arr, int npow) {
         } else if (j == 256) {   // stride 256 alone
             for (int i = threadIdx.x; i < (npow >> 1); i += blockDim.x) {
                 const int l0 = (i & 255) | ((i & ~255) << 1);
-                uint32_t a0 = arr[l0], a1 = arr[l0 | 256];
+                E a0 = arr[l0], a1 = arr[l0 | 256];
                 const bool up = (l0 & kk) == 0;
                 QT_CX(a0, a1)
                 arr[l0] = a0; arr[l0 | 256] = a1;
@@ -491,17 +496,31 @@ __device__ inline void qt_bitonic_sort_w(uint32_t* arr, int npow) {
         // warp pass: strides 128 .. 1 of merge size kk; for kk == 256 every merge from 2 up to 256
         for (int b = warp; b < nblk; b += nwarps) {
             const int base = b << 8, idx0 = base + 4 * lane;
-            uint4* p0 = reinterpret_cast<uint4*>(arr + idx0);
-            uint4* p1 = reinterpret_cast<uint4*>(arr + idx0 + 128);
-            const uint4 x0 = *p0, x1 = *p1;
-            uint32_t v[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-            if (kk == 256) {
-                for (int k = 2; k <= 256; k <<= 1) qt_warp_stages(v, idx0, k, k >> 1, lane);
+            if constexpr (sizeof(E) == 4) {
+                uint4* p0 = reinterpret_cast<uint4*>(arr + idx0);
+                uint4* p1 = reinterpret_cast<uint4*>(arr + idx0 + 128);
+                const uint4 x0 = *p0, x1 = *p1;
+                uint32_t v[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+                if (kk == 256) {
+                    for (int k = 2; k <= 256; k <<= 1) qt_warp_stages(v, idx0, k, k >> 1, lane);
+                } else {
+                    qt_warp_stages(v, idx0, kk, 128, lane);
+                }
+                *p0 = make_uint4(v[0], v[1], v[2], v[3]);
+                *p1 = make_uint4(v[4], v[5], v[6], v[7]);
             } else {
-                qt_warp_stages(v, idx0, kk, 128, lane);
+                ulonglong2* p0 = reinterpret_cast<ulonglong2*>(arr + idx0);
+                ulonglong2* p1 = reinterpret_cast<ulonglong2*>(arr + idx0 + 128);
+                const ulonglong2 x0 = p0[0], x1 = p0[1], x2 = p1[0], x3 = p1[1];
+                uint64_t v[8] = {x0.x, x0.y, x1.x, x1.y, x2.x, x2.y, x3.x, x3.y};
+                if (kk == 256) {
+                    for (int k = 2; k <= 256; k <<= 1) qt_warp_stages(v, idx0, k, k >> 1, lane);
+                } else {
+                    qt_warp_stages(v, idx0, kk, 128, lane);
+                }
+                p0[0] = make_ulonglong2(v[0], v[1]); p0[1] = make_ulonglong2(v[2], v[3]);
+                p1[0] = make_ulonglong2(v[4], v[5]); p1[1] = make_ulonglong2(v[6], v[7]);
             }
-            *p0 = make_uint4(v[0], v[1], v[2], v[3]);
-            *p1 = make_uint4(v[4], v[5], v[6], v[7]);
         }
         __syncthreads();
     }

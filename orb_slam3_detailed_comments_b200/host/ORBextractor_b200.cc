@@ -11,6 +11,11 @@
 // The reference class has no spare member and an inline empty destructor, so the device handle lives in a
 // side table keyed by `this` (three extractors per session: left, right, ini -- Tracking.cc:629-635); the table's
 // destructor releases every handle at process exit, orb_b200_release() releases one earlier.
+//
+// The reference constructor takes no image size.  A handle starts at ORB_B200_MAX_WIDTH x ORB_B200_MAX_HEIGHT; operator() re-creates it
+// for a larger image (each side grows to the larger of the two, never shrinks) and the side table then maps `this` to the new handle,
+// which the stereo and matcher units look up per call.
+#include <algorithm>
 #include <cassert>
 #include <cstdlib>
 #include <cstring>
@@ -34,6 +39,7 @@ namespace {
 struct Registry {
     std::mutex mu;
     std::unordered_map<const void*, orbx_handle*> handles;
+    std::unordered_map<const void*, orbx_config> configs;   // the configuration each handle was created with
     lba_handle* lba = nullptr;
     ~Registry() {
         for (auto& kv : handles) orbx_destroy(kv.second);
@@ -60,6 +66,26 @@ extern "C" void orb_b200_release(const void* extractor) {
     if (it == r.handles.end()) return;
     orbx_destroy(it->second);
     r.handles.erase(it);
+    r.configs.erase(extractor);
+}
+
+// the handle of `extractor`, re-created first when the image is larger than it was sized for
+static orbx_handle* handle_for_image(const void* extractor, int w, int h) {
+    Registry& r = registry();
+    std::lock_guard<std::mutex> lk(r.mu);
+    orbx_handle* cur = r.handles.at(extractor);
+    orbx_config cfg = r.configs.at(extractor);
+    if (w <= cfg.max_width && h <= cfg.max_height) return cur;
+    cfg.max_width = std::max(cfg.max_width, w);
+    cfg.max_height = std::max(cfg.max_height, h);
+    orbx_destroy(cur);            // first: the old and the new workspace need not fit on the device together
+    r.handles.erase(extractor);
+    r.configs.erase(extractor);
+    orbx_handle* grown = nullptr;
+    orb_b200::check(orbx_create(&cfg, &grown), "orbx_create (grow to the image size)");
+    r.handles[extractor] = grown;
+    r.configs[extractor] = cfg;
+    return grown;
 }
 
 extern "C" lba_handle* orb_b200_lba_handle(void) {
@@ -97,6 +123,7 @@ ORBextractor::ORBextractor(int _nfeatures, float _scaleFactor, int _nlevels, int
         auto old = r.handles.find(this);          // an extractor destroyed and another constructed at the same address
         if (old != r.handles.end()) orbx_destroy(old->second);
         r.handles[this] = h;
+        r.configs[this] = cfg;
     }
     mvScaleFactor.resize(nlevels);
     mvInvScaleFactor.resize(nlevels);
@@ -115,7 +142,7 @@ int ORBextractor::operator()(cv::InputArray _image, cv::InputArray /*_mask*/, st
     if (_image.empty()) return -1;
     cv::Mat image = _image.getMat();
     assert(image.type() == CV_8UC1);
-    orbx_handle* h = orb_b200_handle_of(this);
+    orbx_handle* h = handle_for_image(this, image.cols, image.rows);
     static_assert(sizeof(cv::KeyPoint) == sizeof(orbx_keypoint), "cv::KeyPoint layout");
     const int cap = orbx_max_features(h);
     std::vector<cv::KeyPoint> kps(cap);
