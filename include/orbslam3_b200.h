@@ -23,7 +23,8 @@ typedef enum {
     ORB_ERR_EMPTY = -2,        /* empty image: ORBextractor::operator() returns -1 (ORBextractor.cc:1561) */
     ORB_ERR_CUDA = -3,         /* CUDA runtime error; orb_last_error() has the text */
     ORB_ERR_CAPACITY = -4,     /* output or internal capacity exceeded */
-    ORB_ERR_UNSUPPORTED = -5,  /* geometry the reference cannot process either (nIni == 0) or an image side > 4128 px */
+    ORB_ERR_UNSUPPORTED = -5,  /* geometry the reference cannot process either (nIni == 0), an image side > 4128 px, a searched frame
+                                  or keyframe of more than 16 384 feature rows, or a frame-sized shared-memory need above the device's */
     ORB_ERR_NO_DEVICE = -6     /* no CUDA device: there is NO CPU fallback */
 } orb_status;
 

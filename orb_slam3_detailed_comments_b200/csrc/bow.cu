@@ -176,6 +176,11 @@ extern "C" orb_status orbv_transform(orbx_handle* h, const orbv_vocabulary* voc,
     const int nimg = h->last_batch;
     const bool dev = on_device != 0, want_bow = bow_count_out && bow_word_out && bow_weight_out;
     const int maxFeat = h->geom.kpTotal;
+    int npow = 2;
+    while (npow < maxFeat) npow <<= 1;
+    static const size_t bowStatic = static_smem(k_bow_vector);
+    if (want_bow && ((s = check_frame_rows(maxFeat, "frame")) != ORB_OK || (s = check_smem(h, (size_t)npow * 8, bowStatic, "k_bow_vector")) != ORB_OK))
+        return s;
     BowParams P{};
     P.child_off = voc->d_child_off; P.child = voc->d_child; P.ndesc = voc->d_desc; P.nword = voc->d_word; P.nweight = voc->d_weight;
     P.nid_level = voc->L - levelsup;
@@ -199,8 +204,6 @@ extern "C" orb_status orbv_transform(orbx_handle* h, const orbv_vocabulary* voc,
         ORB_LAUNCHED();
     }
     if (want_bow) {
-        int npow = 2;
-        while (npow < maxFeat) npow <<= 1;
         ORB_CUDA(cudaFuncSetAttribute(k_bow_vector, cudaFuncAttributeMaxDynamicSharedMemorySize, npow * 8));
         k_bow_vector<<<nimg, 256, (size_t)npow * 8, st>>>(P);
         ORB_LAUNCHED();

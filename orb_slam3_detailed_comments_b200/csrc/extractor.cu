@@ -330,6 +330,11 @@ static orb_status apply_geometry(orbx_handle* h, int w, int hh) {
         if (k64Groups) ORB_CUDA(qt_k64_set_smem(maxSmem64));   // quadtree_k64.cu (liborbslam3_b200_qt64.so)
     }
     const size_t ordBytes = ((size_t)h->geom.kpTotal + 64) * 4;
+    static const size_t orderStatic = static_smem(k_order);
+    if ((s = check_smem(h, ordBytes, orderStatic, "k_order")) != ORB_OK) {
+        h->cur_w = h->cur_h = -1;
+        return s;
+    }
     ORB_CUDA(cudaFuncSetAttribute(k_order, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(ordBytes, (size_t)1024)));
     h->order_smem_bytes = ordBytes;
     return ORB_OK;
@@ -447,7 +452,7 @@ extern "C" void orbx_destroy(orbx_handle* h) {
     orbr_release(h);
     void* ptrs[] = {h->d_pyr, h->d_blur, h->d_cand, h->d_sort, h->d_lvl_kp, h->d_slot, h->d_cand_cnt, h->d_lvl_cnt,
                     h->d_nkp, h->d_err, h->d_taps, h->d_kps, h->d_desc, h->d_node_scratch, h->d_stage, h->d_po,
-                    h->d_uright, h->d_depth, h->d_sad, h->d_cells, h->d_pat, h->d_blur_frag};
+                    h->d_uright, h->d_depth, h->d_sad, h->d_cells, h->d_pat, h->d_blur_frag, h->d_xl};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (h->h_counts) cudaFreeHost(h->h_counts);

@@ -79,4 +79,39 @@ struct orbx_handle {
     int qt_node_cap = 0, qt_nodes_in_smem = 1;
     size_t qt_node_stride = 0, order_smem_bytes = 0;
     orbr_state* replay = nullptr;   // orbr_submit / orbr_collect state (replay.cu)
+    uint8_t* d_xl = nullptr;        // frame blocks of the matcher's global-memory form (matcher.cu launch_proj)
+    size_t xl_bytes = 0;
+    int smem_optin = 0;             // cudaDevAttrMaxSharedMemoryPerBlockOptin of the handle's device, read on first use
 };
+
+// Rows of one searched frame or keyframe that the matchers accept: an extractor handle's row capacity (n_features + 20 x n_levels)
+// or a host keyframe's feature count.  Feature ids are 16-bit (65 535 would do); the resolve state of the matcher's global-memory
+// form (9 B per row next to 73 KB of query staging), k_bow_vector (8 B x the next power of two) and k_tri_match (14 B per row) fit
+// one CTA's shared memory on an H100 up to this many rows and no further.
+#define ORB_MAX_FRAME_ROWS 16384
+
+inline orb_status check_frame_rows(long long rows, const char* what) {
+    if (rows <= ORB_MAX_FRAME_ROWS) return ORB_OK;
+    return orb::set_error(ORB_ERR_UNSUPPORTED, std::string(what) + " with " + std::to_string(rows) + " feature rows: the matchers take at most " +
+                                                   std::to_string(ORB_MAX_FRAME_ROWS));
+}
+
+inline int smem_optin(orbx_handle* h) {
+    if (h->smem_optin == 0) cudaDeviceGetAttribute(&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->cfg.device);
+    return h->smem_optin;
+}
+
+// A kernel's static shared memory (its __shared__ arrays), which counts against the same per-block limit as the dynamic request
+template <typename... A>
+inline size_t static_smem(void (*kern)(A...)) {
+    cudaFuncAttributes fa{};
+    return cudaFuncGetAttributes(&fa, kern) == cudaSuccess ? fa.sharedSizeBytes : 0;
+}
+
+// A kernel whose dynamic shared memory grows with the frame is refused, before anything is launched, when the device cannot give it
+// that much next to its static arrays: ORB_ERR_UNSUPPORTED with a message rather than a failed launch.
+inline orb_status check_smem(orbx_handle* h, size_t bytes, size_t static_bytes, const char* kernel) {
+    if (bytes + static_bytes <= (size_t)smem_optin(h)) return ORB_OK;
+    return orb::set_error(ORB_ERR_UNSUPPORTED, std::string(kernel) + " needs " + std::to_string(bytes + static_bytes) +
+                                                   " B of shared memory per block; the device allows " + std::to_string(smem_optin(h)));
+}

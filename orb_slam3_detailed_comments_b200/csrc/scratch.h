@@ -12,6 +12,7 @@
 // | `h->d_po` | `orbo_pose_optimization_frames` (it calls the two above), `orbv_transform`, `orbp_distinctive_descriptors`, `orbp_update_normal_and_depth`, `orbm_hamming_knn2` |
 // | `orbr_state::d_buf` | `orbr_submit` (it calls the searches and pose calls above) |
 // | `lba_handle` / `liba_handle` `d_buf`, `h_buf` | `lba_solve*`, `liba_solve` |
+// | `h->d_xl` | the frame blocks of the matcher searches' global-memory form (matcher.cu `launch_proj`) |
 //
 // Captured CUDA graphs hold pointers into these buffers, so a buffer only grows in an eager call: growth inside a capture is refused.
 #pragma once

@@ -300,6 +300,15 @@ static orb_status run_stereo(orbx_handle* hl, orbx_handle* hr, int n_pairs, int 
         return set_error(ORB_ERR_INVALID, "left/right extractors must share device, image size and pyramid");
     if (!(b > 0.f)) return set_error(ORB_ERR_INVALID, "baseline must be positive");
     ORB_CUDA(cudaSetDevice(hl->cfg.device));
+    const char* venv = getenv("ORB_STEREO_VARIANT");      // read at every call: a test can switch variants inside one process
+    const int variant = venv && atoi(venv) == 0 ? 0 : 1;   // default 1 (k_stereo_match_v1) since its round-2 device run
+    const size_t maxRight = hr->geom.kpTotal, H = hr->geom.lv[0].h;
+    const size_t smem1 = 13 * maxRight + 4 * (2 * H + 2) + 64, smem = 9 * maxRight + 16, smem2 = 4 * (size_t)hl->geom.kpTotal + 16;
+    static const size_t v1Static = static_smem(k_stereo_match_v1), v0Static = static_smem(k_stereo_match), medStatic = static_smem(k_stereo_median);
+    orb_status s;
+    if ((s = variant == 1 ? check_smem(hl, smem1, v1Static, "k_stereo_match_v1") : check_smem(hl, smem, v0Static, "k_stereo_match")) != ORB_OK ||
+        (s = check_smem(hl, smem2, medStatic, "k_stereo_median")) != ORB_OK)
+        return s;
     cudaStream_t st = hl->stream;
     if (hr != hl) {   // order after the right extractor's work
         ORB_CUDA(cudaEventRecord(hr->ev_fork, hr->stream));
@@ -312,22 +321,16 @@ static orb_status run_stereo(orbx_handle* hl, orbx_handle* hr, int n_pairs, int 
     P.bf = bf; P.b = b;
     P.uright = hl->d_uright; P.depth = hl->d_depth; P.sad = hl->d_sad;
     P.maxRight = hr->geom.kpTotal;
-    const char* venv = getenv("ORB_STEREO_VARIANT");      // read at every call: a test can switch variants inside one process
-    const int variant = venv && atoi(venv) == 0 ? 0 : 1;   // default 1 (k_stereo_match_v1) since its round-2 device run
     if (variant == 1) {
-        const int H = hr->geom.lv[0].h;
-        const size_t smem1 = 13 * (size_t)P.maxRight + 4 * (2 * (size_t)H + 2) + 64;
         ORB_CUDA(cudaFuncSetAttribute(k_stereo_match_v1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem1, (size_t)1024)));
         dim3 grid1((hl->geom.kpTotal + ST1_THREADS - 1) / ST1_THREADS, n_pairs);
         launch_p(k_stereo_match_v1, grid1, dim3(ST1_THREADS), smem1, st, P, hl->geom, hr->geom);
     } else {
-        const size_t smem = 9 * (size_t)P.maxRight + 16;
         ORB_CUDA(cudaFuncSetAttribute(k_stereo_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem, (size_t)1024)));
         dim3 grid((hl->geom.kpTotal + ST_WARPS - 1) / ST_WARPS, n_pairs);
         k_stereo_match<<<grid, ST_WARPS * 32, smem, st>>>(P, hl->geom, hr->geom);
     }
     ORB_LAUNCHED();
-    const size_t smem2 = 4 * (size_t)hl->geom.kpTotal + 16;
     ORB_CUDA(cudaFuncSetAttribute(k_stereo_median, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem2, (size_t)1024)));
     launch_p(k_stereo_median, dim3(n_pairs), dim3(256), smem2, st, P);
     ORB_LAUNCHED();

@@ -156,7 +156,8 @@ __global__ void __launch_bounds__(256) k_tri_rotation(const __grid_constant__ Tr
 extern "C" orb_status orbm_search_triangulation(orbx_handle* h, const orbm_triangulation* T, int32_t* match12_out,
                                                 int32_t* nmatches_out) {
     if (!h || !T || !match12_out || T->n_queries < 0 || T->n2 < 0) return set_error(ORB_ERR_INVALID, "bad arguments");
-    if (T->n2 > 65535) return set_error(ORB_ERR_UNSUPPORTED, "more than 65535 features in a keyframe");
+    orb_status s;
+    if ((s = check_frame_rows(T->n2, "keyframe")) != ORB_OK) return s;
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     const int nq = T->n_queries, N2 = T->n2;
     if (nmatches_out) *nmatches_out = 0;
@@ -175,6 +176,9 @@ extern "C" orb_status orbm_search_triangulation(orbx_handle* h, const orbm_trian
         P.sigma2[l] = l < h->cfg.n_levels ? h->sigma2[l] : 1.f;
     }
     P.coarse = T->coarse; P.checkOri = T->check_orientation;
+    const size_t smem = (size_t)N2 * 14 + 16;
+    static const size_t triStatic = static_smem(k_tri_match);
+    if ((s = check_smem(h, smem, triStatic, "k_tri_match")) != ORB_OK) return s;
     auto layout = [&](Carve& c) {
         P.kp1 = stage_in(c, T->kp1, nq, false); P.desc1 = stage_in(c, T->desc1, (size_t)nq * 32, false);
         P.node1 = stage_in(c, T->node1, nq, false); P.stereo1 = stage_in(c, T->stereo1, nq, false);
@@ -184,9 +188,7 @@ extern "C" orb_status orbm_search_triangulation(orbx_handle* h, const orbm_trian
         P.bins = c.take<int>(nq);
         P.nmatches = c.take<int>(1);
     };
-    const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
-    if (s != ORB_OK) return s;
-    const size_t smem = (size_t)N2 * 14 + 16;
+    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
     ORB_CUDA(cudaFuncSetAttribute(k_tri_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem, (size_t)1024)));
     k_tri_match<<<(nq + TRI_QPB - 1) / TRI_QPB, TRI_WARPS * 32, smem, h->stream>>>(P);
     ORB_LAUNCHED();
