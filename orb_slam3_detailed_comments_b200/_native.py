@@ -16,17 +16,6 @@ SOURCES = ["extractor.cu", "stereo.cu", "matcher.cu", "triangulation.cu", "lba.c
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
-# k_blur_mma (the tensor-core blur) is its own library next to the main one, which links it and finds it through RUNPATH $ORIGIN
-BLUR_SOURCES = ["blur_mma.cu"]
-BLUR_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_blur.so")
-# k_quadtree_v1_k64 (DistributeOctTree on the 64-bit element, regions over 2048 px) likewise
-QT64_SOURCES = ["quadtree_k64.cu"]
-QT64_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_qt64.so")
-# the matcher's global-memory form (frames whose shared-memory form does not fit a CTA) likewise
-MATCH_XL_SOURCES = ["matcher_xl.cu"]
-MATCH_XL_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_match_xl.so")
-LINK_FLAGS = ["-L", os.path.dirname(BLUR_LIB_PATH), "-lorbslam3_b200_blur", "-lorbslam3_b200_qt64", "-lorbslam3_b200_match_xl",
-              "-Xlinker", "-rpath,$ORIGIN"]
 
 KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"),
                      ("response", "<f4"), ("octave", "<i4"), ("class_id", "<i4")])
@@ -37,20 +26,17 @@ class OrbError(RuntimeError):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200_blur.so, lib/liborbslam3_b200_qt64.so,
-    lib/liborbslam3_b200_match_xl.so and lib/liborbslam3_b200.so, which links the other three (nvcc cross-compiles on CPU)."""
-    deps = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)] + [os.path.join(_PKG, "..", "include", "orbslam3_b200.h")]
+    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so (nvcc cross-compiles on CPU)."""
+    deps = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)] + [os.path.join(_PKG, "..", "include", "orbslam3_b200.h"),
+                                                                   os.path.abspath(__file__)]   # the recipe itself
     if os.environ.get("ORB_LIB_PATH"):
         return LIB_PATH                       # an explicitly chosen build is never rebuilt
+    if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
+        return LIB_PATH
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     os.makedirs(os.path.dirname(LIB_PATH), exist_ok=True)
-    for out, sources, link in [(BLUR_LIB_PATH, BLUR_SOURCES, []), (QT64_LIB_PATH, QT64_SOURCES, []), (MATCH_XL_LIB_PATH, MATCH_XL_SOURCES, []),
-                               (LIB_PATH, SOURCES, LINK_FLAGS)]:
-        if (not force and os.path.exists(out)
-                and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps)):
-            continue
-        cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", out] + [os.path.join(_CSRC, s) for s in sources] + link
-        subprocess.check_call(cmd)
+    subprocess.check_call([nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB_PATH] +
+                          [os.path.join(_CSRC, s) for s in SOURCES])
     return LIB_PATH
 
 

@@ -327,7 +327,8 @@ static orb_status apply_geometry(orbx_handle* h, int w, int hh) {
         ORB_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxSmem));
         ORB_CUDA(cudaFuncSetAttribute(k_quadtree_v1<QT_THREADS, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxSmem));
         ORB_CUDA(cudaFuncSetAttribute(k_quadtree_v1<1024, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxSmem));
-        if (k64Groups) ORB_CUDA(qt_k64_set_smem(maxSmem64));   // quadtree_k64.cu (liborbslam3_b200_qt64.so)
+        if (k64Groups)
+            ORB_CUDA(cudaFuncSetAttribute(k_quadtree_v1_k64<QT_K64_THREADS, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxSmem64));
     }
     const size_t ordBytes = ((size_t)h->geom.kpTotal + 64) * 4;
     static const size_t orderStatic = static_smem(k_order);
@@ -545,15 +546,11 @@ static orb_status run_pipeline(orbx_handle* h, int batch, int lap0, int lap1) {
         // 1024 threads per CTA for the group with level 0 and, after a 64-bit group, for the first 32-bit group (the largest levels of
         // each form).  The 64-bit group always holds level 0.
         const bool wide = h->qt_variant == 1 && (gi == 0 || (gi == 1 && h->qt_groups[0].k64));
-        if (Q.k64)   // k_quadtree_v1_k64 lives in liborbslam3_b200_qt64.so: its launch error comes back from there
-            ORB_CUDA(launch_quadtree_k64(batch * (Q.level_end - Q.level_begin), Q.smem, qs, g, batch, Q.level_begin, h->d_cand, h->d_cand_cnt,
-                                         h->d_sort, (char*)h->d_node_scratch, (int64_t)h->qt_node_stride, Q.sort_cap, h->qt_nodes_in_smem,
-                                         h->qt_node_cap, h->d_lvl_kp, h->d_lvl_cnt, h->d_err));
-        else
-            launch_p(h->qt_variant == 0 ? k_quadtree : wide ? k_quadtree_v1<1024, 1> : k_quadtree_v1<QT_THREADS, 4>,
-                     dim3(batch * (Q.level_end - Q.level_begin)), dim3(wide ? 1024 : QT_THREADS), Q.smem, qs,
-                     g, batch, Q.level_begin, h->d_cand, h->d_cand_cnt, h->d_sort, (char*)h->d_node_scratch,
-                     (int64_t)h->qt_node_stride, Q.sort_cap, h->qt_nodes_in_smem, h->qt_node_cap, h->d_lvl_kp, h->d_lvl_cnt, h->d_err);
+        launch_p(Q.k64 ? k_quadtree_v1_k64<QT_K64_THREADS, 1>
+                       : h->qt_variant == 0 ? k_quadtree : wide ? k_quadtree_v1<1024, 1> : k_quadtree_v1<QT_THREADS, 4>,
+                 dim3(batch * (Q.level_end - Q.level_begin)), dim3(Q.k64 ? QT_K64_THREADS : wide ? 1024 : QT_THREADS), Q.smem, qs,
+                 g, batch, Q.level_begin, h->d_cand, h->d_cand_cnt, h->d_sort, (char*)h->d_node_scratch,
+                 (int64_t)h->qt_node_stride, Q.sort_cap, h->qt_nodes_in_smem, h->qt_node_cap, h->d_lvl_kp, h->d_lvl_cnt, h->d_err);
         ORB_LAUNCHED();
         if (gi > 0) {
             cudaEventRecord(h->ev_join[gi - 1], qs);
@@ -575,7 +572,7 @@ static orb_status run_pipeline(orbx_handle* h, int batch, int lap0, int lap1) {
             tiles += bp.tilesX[l] * ((g.lv[l].h + BM_TH - 1) / BM_TH);
         }
         bp.tileBase[g.nlevels] = tiles;
-        ORB_CUDA(launch_blur_mma(g, bp, tiles, batch, st));
+        k_blur_mma<<<dim3(tiles, batch), 256, 0, st>>>(g, bp);
     } else if (h->blur_variant == 1) k_blur<true><<<dim3(g.totalTiles, batch), 256, 0, st>>>(g);    // horizontal pass by IDP.4A
     else k_blur<false><<<dim3(g.totalTiles, batch), 256, 0, st>>>(g);
     ORB_LAUNCHED();

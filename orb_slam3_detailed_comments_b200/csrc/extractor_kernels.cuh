@@ -437,6 +437,11 @@ __global__ void __launch_bounds__(QT_THREADS) k_quadtree(const __grid_constant__
 template <int MAXT, int MINB>
 __global__ void __launch_bounds__(MAXT, MINB) k_quadtree_v1(QT_V1_PARAMS) { qt_v1_body<uint32_t>(QT_V1_ARGS); }
 
+// k_quadtree_v1 on the 64-bit, 12-depth sort element, for the level group whose region side exceeds 2048 px (it always holds level 0;
+// levels of 2048 px or less never run it).  Launched as <QT_K64_THREADS, 1>.
+template <int MAXT, int MINB>
+__global__ void __launch_bounds__(MAXT, MINB) k_quadtree_v1_k64(QT_V1_PARAMS) { qt_v1_body<uint64_t>(QT_V1_ARGS); }
+
 // ---------------------------------------------------------------------------------------------
 // K3b  output slot of every keypoint (ORBextractor.cc:1656-1678): emission order is level-major;
 // keypoints whose scaled x lies in [lap0, lap1] fill the output from the back, the others from the

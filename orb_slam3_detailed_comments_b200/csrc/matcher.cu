@@ -19,8 +19,8 @@
 // stored list so that its best / second best can no longer be known, the resolve warp rescans that
 // query with the mask applied (exact slow path).
 //
-// The kernel bodies live in matcher_core.cuh.  This file builds the shared-memory form, which stages the searched frame in each CTA;
-// matcher_xl.cu builds the global-memory form for frames too large for that (launch_proj picks one per call).
+// The kernel bodies live in matcher_core.cuh.  This file builds them in two forms: the shared-memory form, which stages the searched
+// frame in each CTA, and the global-memory form (*_xl) for frames too large for that (launch_proj picks one per call).
 #include <algorithm>
 #include <vector>
 
@@ -119,6 +119,37 @@ __global__ void __launch_bounds__(PR_THREADS) k_proj_resolve_par(const __grid_co
 #include "matcher_resolve_par.inc"
 }
 
+// ---- the same kernels, global-memory form ---------------------------------------------------------------------------------
+// One CTA per frame writes the FrameFeat block (and for the grid searches the GridFeat block, after k_frame_grid) that the
+// shared-memory form stages in every CTA.
+__global__ void __launch_bounds__(1024) k_stage_frames_xl(const __grid_constant__ ProjParams P, const GlobalFrame S) {
+    const int frame = blockIdx.x;
+    FrameFeat F;
+    int N, row0;
+    stage_frame(P, P.frame_image[frame], S.featBlocks + (size_t)frame * S.featStride, F, N, row0);
+    if (S.gridBlocks) {
+        GridFeat GF;
+        stage_grid(P, frame, S.gridBlocks + (size_t)frame * S.gridStride, GF, N, row0);
+    }
+}
+
+template <int G>
+__global__ void __launch_bounds__(PM_WARPS * 32) k_proj_candidates_grp_xl(const __grid_constant__ ProjParams P, const GlobalFrame S) {
+    proj_candidates_grp_body<G>(P, S);
+}
+
+__global__ void __launch_bounds__(PM_WARPS * 32) k_proj_candidates_xl(const __grid_constant__ ProjParams P, const GlobalFrame S) {
+    proj_candidates_body(P, S);
+}
+
+__global__ void __launch_bounds__(256) k_proj_resolve_xl(const __grid_constant__ ProjParams P, const GlobalFrame S) {
+#include "matcher_resolve.inc"
+}
+
+__global__ void __launch_bounds__(PR_THREADS) k_proj_resolve_par_xl(const __grid_constant__ ProjParams P, const GlobalFrame S) {
+#include "matcher_resolve_par.inc"
+}
+
 // ---- Frame::isInFrustum (src/Frame.cc:667-720): one thread per candidate map point ------------------------------------
 struct FrustumParams {
     const int* poff;           // [n_frames + 1]
@@ -185,7 +216,7 @@ __global__ void __launch_bounds__(256) k_in_frustum(const __grid_constant__ Frus
 // host side
 // ------------------------------------------------------------------------------------------------
 // Runs one search.  The call's shared-memory need (the largest block its kernels ask for) decides the form, once per call: the
-// shared-memory form whenever the device can give it, else the global-memory form (matcher_xl.cu), whose frame blocks live in
+// shared-memory form whenever the device can give it, else the global-memory form (*_xl), whose frame blocks live in
 // h->d_xl and whose kernels keep only the per-feature resolve state in shared memory.  Both compute the same matches.
 static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int max_q_per_frame) {
     cudaStream_t st = h->stream;
@@ -223,7 +254,7 @@ static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int m
         ORB_LAUNCHED();
     }
     if (global) {
-        ORB_CUDA(launch_proj_xl(PXL_STAGE, dim3(n_frames), 0, st, P, S));
+        launch_p(k_stage_frames_xl, dim3(n_frames), dim3(1024), 0, st, P, S);
         ORB_LAUNCHED();
     }
     // modes 0 / 1 (the two per-frame searches): G lanes per query (ORB_PROJ_LANES = 4 | 8 | 16; 32 = the warp-per-query kernel)
@@ -235,8 +266,9 @@ static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int m
         P.qpb = envQpb > 0 ? envQpb : (P.mode == 0 ? 128 : 64);
         dim3 grid((max_q_per_frame + P.qpb - 1) / P.qpb, n_frames);
         if (global) {
+            auto kern = lanes == 4 ? k_proj_candidates_grp_xl<4> : (lanes == 8 ? k_proj_candidates_grp_xl<8> : k_proj_candidates_grp_xl<16>);
             if (grid.x > 0) {
-                ORB_CUDA(launch_proj_xl(lanes == 4 ? PXL_CAND_G4 : (lanes == 8 ? PXL_CAND_G8 : PXL_CAND_G16), grid, 0, st, P, S));
+                launch_p(kern, grid, dim3(PM_WARPS * 32), 0, st, P, S);
                 ORB_LAUNCHED();
             }
         } else {
@@ -251,7 +283,7 @@ static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int m
         dim3 grid((max_q_per_frame + PM_QPB - 1) / PM_QPB, n_frames);
         if (global) {
             if (grid.x > 0) {
-                ORB_CUDA(launch_proj_xl(PXL_CAND, grid, 0, st, P, S));
+                launch_p(k_proj_candidates_xl, grid, dim3(PM_WARPS * 32), 0, st, P, S);
                 ORB_LAUNCHED();
             }
         } else {
@@ -263,12 +295,13 @@ static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int m
         }
     }
     if (global) {
-        ORB_CUDA(proj_xl_set_smem(psm - fsm, rsm - fsm));
+        ORB_CUDA(cudaFuncSetAttribute(k_proj_resolve_par_xl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(psm - fsm)));
+        ORB_CUDA(cudaFuncSetAttribute(k_proj_resolve_xl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(rsm - fsm)));
         if (P.seqFlag) {
-            ORB_CUDA(launch_proj_xl(PXL_RESOLVE_PAR, dim3(n_frames), psm - fsm, st, P, S));
+            launch_p(k_proj_resolve_par_xl, dim3(n_frames), dim3(PR_THREADS), psm - fsm, st, P, S);
             ORB_LAUNCHED();
         }
-        ORB_CUDA(launch_proj_xl(PXL_RESOLVE, dim3(n_frames), rsm - fsm, st, P, S));
+        launch_p(k_proj_resolve_xl, dim3(n_frames), dim3(256), rsm - fsm, st, P, S);
         ORB_LAUNCHED();
         ORB_CUDA(cudaGetLastError());
         return ORB_OK;

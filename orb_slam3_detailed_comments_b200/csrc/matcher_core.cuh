@@ -1,11 +1,10 @@
 // matcher_core.cuh -- the device code of the ORBmatcher searches (matcher.cu), written once for both places the searched frame's
 // features can live:
 //   * SmemFrame: each CTA stages the frame into its own shared memory (FrameFeat 23 B, GridFeat 17 B per feature).  The kernels
-//     k_proj_candidates[_grp], k_proj_resolve_par and k_proj_resolve of liborbslam3_b200.so (matcher.cu).
+//     k_proj_candidates[_grp], k_proj_resolve_par and k_proj_resolve of matcher.cu.
 //   * GlobalFrame: k_stage_frames_xl writes the same FrameFeat / GridFeat blocks once per frame into global scratch and the kernels
 //     read them from there (L2-resident: ~650 KB per frame at 16 384 features); only the per-feature resolve state stays in shared
-//     memory.  The *_xl kernels of liborbslam3_b200_match_xl.so (matcher_xl.cu), which liborbslam3_b200.so links, so the main
-//     library keeps exactly its kernels and machine code.
+//     memory.  The *_xl kernels of matcher.cu.
 // launch_proj (matcher.cu) runs the shared-memory form whenever a call's shared-memory need fits the device's opt-in limit.
 #pragma once
 #include "common.cuh"
@@ -689,12 +688,5 @@ __device__ __forceinline__ int pr_decide(const ProjParams& P, const FrameFeat& F
     }
     return bestIdx;
 }
-
-// ---- the global-memory form: matcher_xl.cu (liborbslam3_b200_match_xl.so) ------------------------------------------------------
-enum ProjXlKernel { PXL_STAGE, PXL_CAND_G4, PXL_CAND_G8, PXL_CAND_G16, PXL_CAND, PXL_RESOLVE_PAR, PXL_RESOLVE };
-// Sets the dynamic shared-memory limits of the two resolve kernels, and launches one kernel of the form on `st` (grid `grid`, its
-// own block size); each returns the CUDA error, if any.
-cudaError_t proj_xl_set_smem(size_t resolve_par_bytes, size_t resolve_bytes);
-cudaError_t launch_proj_xl(ProjXlKernel kernel, dim3 grid, size_t smem, cudaStream_t st, const ProjParams& P, const GlobalFrame& S);
 
 }  // namespace orb

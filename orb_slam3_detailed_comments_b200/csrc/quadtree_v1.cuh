@@ -1,7 +1,6 @@
 // quadtree_v1.cuh -- the body of k_quadtree_v1 (DistributeOctTree, one CTA per (level, image); quadtree_core.cuh), written once for
-// both sort elements: k_quadtree_v1 (extractor_kernels.cuh, 32-bit element, regions up to 2048 px) and k_quadtree_v1_k64
-// (quadtree_k64.cu, 64-bit element, regions up to 4096 px).  k_quadtree_v1_k64 is built into its own library, liborbslam3_b200_qt64.so,
-// which liborbslam3_b200.so links, so the main library keeps exactly its GPU-validated kernels and machine code.
+// both sort elements: k_quadtree_v1 (32-bit element, regions up to 2048 px) and k_quadtree_v1_k64 (64-bit element, regions up to
+// 4096 px), both in extractor_kernels.cuh.
 #pragma once
 #include "common.cuh"
 #include "quadtree_core.cuh"
@@ -80,13 +79,5 @@ __device__ __forceinline__ void qt_v1_body(const ExtractGeom& g, int batch, int 
 // k_quadtree_v1_k64 runs 512 threads per CTA: the 128 registers a thread may then hold keep the 64-bit sort network out of local
 // memory (at 1024 threads, 64 registers, it spills).
 #define QT_K64_THREADS 512
-
-// quadtree_k64.cu: sets k_quadtree_v1_k64's dynamic shared-memory limit, and launches it on `st` (grid `blocks`, QT_K64_THREADS
-// threads) with the arguments of k_quadtree_v1; each returns the CUDA error, if any.
-cudaError_t qt_k64_set_smem(size_t bytes);
-cudaError_t launch_quadtree_k64(int blocks, size_t smem, cudaStream_t st, const ExtractGeom& g, int batch, int levelBegin,
-                                const uint32_t* cand, const int* candCnt, uint32_t* sortScratch, char* nodeScratch,
-                                int64_t nodeScratchStride, int sortCapSmem, int nodesInSmem, int nodeCapMax, uint32_t* lvlKp, int* lvlCnt,
-                                int* err);
 
 }  // namespace orb

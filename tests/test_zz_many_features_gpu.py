@@ -1,5 +1,5 @@
 """GPU tier: frames and keyframes of up to 16 384 feature rows through the matchers, bit for bit against the oracle.  Frames whose
-shared-memory form does not fit a CTA run the global-memory form (liborbslam3_b200_match_xl.so); which form ran is read from the
+shared-memory form does not fit a CTA run the global-memory form (the *_xl kernels); which form ran is read from the
 library's launch counter (the global form adds k_stage_frames_xl).  Covered: ORB-SLAM3's 5x-feature monocular initialisation on a
 EuRoC-shaped frame (F2 on the device and as host arrays); KITTI-shaped 1241x376 monocular frames at 10 000 features (both per-frame
 searches, with and without the isInFrustum mask, SearchByBoW(KF, F), relocalisation); a 3840x2160 stereo batch at 16 000 features

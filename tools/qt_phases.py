@@ -16,7 +16,7 @@ PROF = os.path.join(ROOT, "orb_slam3_detailed_comments_b200", "lib", "liborbslam
 if "--build" in sys.argv:
     from orb_slam3_detailed_comments_b200 import _native as N
     srcs = [os.path.join(N._CSRC, s) for s in N.SOURCES]
-    subprocess.check_call([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")] + N.NVCC_FLAGS + ["-DQT_PROFILE", "-o", PROF] + srcs + N.LINK_FLAGS)
+    subprocess.check_call([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")] + N.NVCC_FLAGS + ["-DQT_PROFILE", "-o", PROF] + srcs)
     print("built", PROF)
     sys.exit(0)
 
