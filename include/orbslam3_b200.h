@@ -638,6 +638,16 @@ orb_status liba_link_information(const float* C15x15, int32_t oldest, double* in
  * host memory makes the copies asynchronous; a host thread that keeps several handles in flight (submit on handles
  * k+1 .. k+H-1 before collecting handle k) overlaps uploads, kernels and downloads without further threads.
  * One step per handle may be in flight.  Images: 2 * n_frames, left eye of frame p = image 2p, right eye = image 2p + 1.
+ *
+ * Monocular step (orbr_step::monocular != 0): what Tracking::GrabImageMonocular -> Frame::Frame(monocular) -> Track does per frame
+ * for a rectified camera.  Image f is frame f (n_frames images, n_frames <= max_batch).  Each image goes through
+ * ORBextractor::operator() with vLappingArea = {0, 1000} (Frame.cc:380), so keypoints are back-filled as the reference orders them;
+ * Frame::UndistortKeyPoints is an identity copy for a camera with zero distortion and is not run.  ComputeStereoMatches does not run:
+ * every feature has mvuRight = mvDepth = -1, so both searches and PoseOptimization take their monocular branches and bf / b are
+ * ignored.  TrackWithMotionModel passes bMono = true for a monocular sensor (Tracking.cc:3389-3443), so the last-frame search
+ * never looks forward or backward: every last->direction[f] must be 0 (ORBmatcher.cc:1967-1971).  frame_image indexes
+ * [0, n_frames).  The searches, PoseOptimization and the chained flow keep their meaning.  orbr_collect returns n / offsets with
+ * n_frames / n_frames + 1 entries and fills uright / depth with -1.
  * ---------------------------------------------------------------------------------------------- */
 /* The chained data flow of one tracked frame (Tracking.cc:3389-3522, 4010-4062) instead of two independent searches with precomputed
  * projections: the motion-model search and its PoseOptimization run first; the features whose map point came out an outlier are released
@@ -658,7 +668,7 @@ typedef struct {
 
 typedef struct {
     int32_t n_frames;
-    const uint8_t* images;               /* HOST: 2 * n_frames images */
+    const uint8_t* images;               /* HOST: 2 * n_frames images (n_frames with monocular) */
     int32_t width, height, stride;       /* stride in bytes between rows */
     size_t image_stride_bytes;           /* between consecutive images */
     float bf, b;                         /* Frame::mbf, Frame::mb */
@@ -674,16 +684,17 @@ typedef struct {
     const float* local_world_pos;        /* [nq_local][3] GetWorldPos() of the local-map entries (with pose_optimization) */
     const orbr_chain* chain;             /* NULL, or the chained flow: needs `last` and `pose`, `local` must be NULL; PoseOptimization runs after both
                                             searches whatever pose_optimization says; local_* results are indexed by the chain's map points */
+    int32_t monocular;                   /* != 0: n_frames images, one per frame (Frame's monocular constructor), instead of 2 * n_frames stereo eyes */
 } orbr_step;
 
 typedef struct {                         /* HOST result buffers; any pointer may be NULL (that result is not copied back) */
     int32_t cap_rows;                    /* capacity, in rows, of every per-row / per-edge array below */
     orbx_keypoint* keypoints;            /* compact rows of the whole batch, image after image (mvKeys) */
     uint8_t* descriptors;                /* [rows][32] (mDescriptors) */
-    float* uright;                       /* [rows] mvuRight (left-eye rows) */
-    float* depth;                        /* [rows] mvDepth */
-    int32_t* n;                          /* [2 n_frames] keypoints per image */
-    int32_t* offsets;                    /* [2 n_frames + 1] first row of every image */
+    float* uright;                       /* [rows] mvuRight (left-eye rows; -1 in a monocular step) */
+    float* depth;                        /* [rows] mvDepth (-1 in a monocular step) */
+    int32_t* n;                          /* [2 n_frames] keypoints per image (n_frames in a monocular step) */
+    int32_t* offsets;                    /* [2 n_frames + 1] first row of every image (n_frames + 1 in a monocular step) */
     int32_t* last_feature_match;         /* [rows] as orbm_search_last_frame */
     int32_t* last_nmatches;              /* [n_frames] */
     int32_t* local_match;                /* [nq_local] as orbm_search_local_points */

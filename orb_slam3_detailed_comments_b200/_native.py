@@ -96,7 +96,8 @@ class orbr_step(C.Structure):
                 ("image_stride_bytes", C.c_size_t), ("bf", C.c_float), ("b", C.c_float), ("last", C.POINTER(orbm_last_queries)),
                 ("th_last", C.c_float), ("check_orientation_last", C.c_int32), ("local", C.POINTER(orbm_local_queries)),
                 ("th_local", C.c_float), ("nnratio_local", C.c_float), ("far_points", C.c_int32), ("th_far", C.c_float),
-                ("pose_optimization", C.c_int32), ("pose", C.c_void_p), ("local_world_pos", C.c_void_p), ("chain", C.POINTER(orbr_chain))]
+                ("pose_optimization", C.c_int32), ("pose", C.c_void_p), ("local_world_pos", C.c_void_p), ("chain", C.POINTER(orbr_chain)),
+                ("monocular", C.c_int32)]
 
 
 class orbr_results(C.Structure):

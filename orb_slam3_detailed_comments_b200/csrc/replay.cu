@@ -1,13 +1,15 @@
-// replay.cu -- batched sequence replay: the tracking-thread step of a batch of stereo frames through ONE pair of calls,
+// replay.cu -- batched sequence replay: the tracking-thread step of a batch of stereo or monocular frames through ONE pair of calls,
 // host buffers in / host buffers out (include/orbslam3_b200.h: orbr_submit / orbr_collect).
 //
 // What the reference's Tracking thread does per frame -- Frame::Frame (both eyes through ORBextractor::operator(),
 // Frame.cc:136-141; ComputeStereoMatches, Frame.cc:1102), TrackWithMotionModel (SearchByProjection(cur, last), PoseOptimization,
 // Tracking.cc:3389-3443), TrackLocalMap (SearchByProjection(F, local map points), PoseOptimization, Tracking.cc:4052, 3522) --
 // queued for n_frames frames at once on the handle's stream: one H2D of the images, one H2D per query array, the kernels, and
-// the small count tables back.  orbr_submit returns as soon as everything is queued; orbr_collect waits for the counts, reads
-// back exactly the rows the batch produced and waits once more.  A host thread that keeps several handles in flight
-// (submit k+1 .. k+H-1 before collect k) overlaps uploads, kernels and downloads of different handles without more threads.
+// the small count tables back.  A monocular step (orbr_step::monocular) extracts one image per frame with vLappingArea = {0, 1000}
+// (Frame.cc:380) and skips ComputeStereoMatches; everything after the extraction is shared.  orbr_submit returns as soon as
+// everything is queued; orbr_collect waits for the counts, reads back exactly the rows the batch produced and waits once more.
+// A host thread that keeps several handles in flight (submit k+1 .. k+H-1 before collect k) overlaps uploads, kernels and
+// downloads of different handles without more threads.
 #include <string.h>
 
 #include <algorithm>
@@ -24,7 +26,8 @@ struct orbr_state {
     uint8_t* d_buf = nullptr;
     size_t bytes = 0;
     bool pending = false;
-    int n_frames = 0, nq_last = 0, nq_local = 0, with_po = 0;
+    int n_frames = 0, nimg = 0, nq_last = 0, nq_local = 0, with_po = 0;
+    bool mono = false;
     cudaEvent_t ev_counts = nullptr;
     // result pointers inside d_buf
     int *d_fm = nullptr, *d_nm_last = nullptr, *d_match = nullptr, *d_nm_local = nullptr;
@@ -124,11 +127,13 @@ void orbr_release(orbx_handle* h) {   // called by orbx_destroy
 
 extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const orbr_step* S) {
     if (!h || !cam || !S || S->n_frames < 1 || !S->images) return set_error(ORB_ERR_INVALID, "bad arguments");
-    if (2 * S->n_frames > h->cfg.max_batch) return set_error(ORB_ERR_INVALID, "2 * n_frames exceeds the handle's max_batch");
+    const bool mono = S->monocular != 0;
+    const int nf = S->n_frames, nimg = mono ? nf : 2 * nf;   // monocular: image f is frame f; stereo: eyes 2f, 2f + 1
+    if (nimg > h->cfg.max_batch)
+        return set_error(ORB_ERR_INVALID, mono ? "n_frames exceeds the handle's max_batch" : "2 * n_frames exceeds the handle's max_batch");
     if (h->capturing) return set_error(ORB_ERR_INVALID, "orbr_submit cannot run inside a graph capture");
     const orbm_last_queries* QL = S->last;
     const orbm_local_queries* QC = S->local;
-    const int nf = S->n_frames;
     if (QL && (QL->n_frames != nf || !QL->frame_image || !QL->query_offset || !QL->Tcw || !QL->direction)) return set_error(ORB_ERR_INVALID, "bad last-frame query set");
     if (QC && (QC->n_frames != nf || !QC->frame_image || !QC->query_offset)) return set_error(ORB_ERR_INVALID, "bad local-map query set");
     const orbr_chain* CH = S->chain;
@@ -153,11 +158,13 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         }
     for (int f = 0; f < nf; ++f) {
         if (QL) {
-            if (QL->query_offset[f + 1] < QL->query_offset[f] || QL->frame_image[f] < 0 || QL->frame_image[f] >= 2 * nf) return set_error(ORB_ERR_INVALID, "bad frame table");
+            if (QL->query_offset[f + 1] < QL->query_offset[f] || QL->frame_image[f] < 0 || QL->frame_image[f] >= nimg) return set_error(ORB_ERR_INVALID, "bad frame table");
+            // bMono: the monocular search never looks forward or backward (ORBmatcher.cc:1967-1971)
+            if (mono && QL->direction[f] != 0) return set_error(ORB_ERR_INVALID, "a monocular step needs direction 0 for every frame");
             maxqL = std::max(maxqL, QL->query_offset[f + 1] - QL->query_offset[f]);
         }
         if (QC) {
-            if (QC->query_offset[f + 1] < QC->query_offset[f] || QC->frame_image[f] < 0 || QC->frame_image[f] >= 2 * nf) return set_error(ORB_ERR_INVALID, "bad frame table");
+            if (QC->query_offset[f + 1] < QC->query_offset[f] || QC->frame_image[f] < 0 || QC->frame_image[f] >= nimg) return set_error(ORB_ERR_INVALID, "bad frame table");
             maxqC = std::max(maxqC, QC->query_offset[f + 1] - QC->query_offset[f]);
         }
     }
@@ -200,10 +207,11 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         r->h_eoff_cap = 2 * (nf + 1);
     }
     cudaStream_t st = h->stream;
-    // ---- both eyes of every frame through the extractor, then ComputeStereoMatches ----
-    s = orbx_extract_batch(h, S->images, 2 * nf, S->width, S->height, S->stride, S->image_stride_bytes, 0, 0, nullptr, nullptr);
+    // ---- both eyes of every frame through the extractor, then ComputeStereoMatches; or the one image of every monocular frame
+    //      with vLappingArea = {0, 1000} (Frame.cc:380) and no stereo: mvuRight stays -1 for the searches and PoseOptimization ----
+    s = orbx_extract_batch(h, S->images, nimg, S->width, S->height, S->stride, S->image_stride_bytes, 0, mono ? 1000 : 0, nullptr, nullptr);
     if (s != ORB_OK) return s;
-    if ((s = orbm_stereo_batch(h, nf, S->bf, S->b)) != ORB_OK) return s;
+    if (!mono && (s = orbm_stereo_batch(h, nf, S->bf, S->b)) != ORB_OK) return s;
     auto up = [&](void* dst, const void* src, size_t bytes) -> orb_status {
         if (src && bytes) ORB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
         return ORB_OK;
@@ -303,7 +311,8 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     ORB_CUDA(cudaMemcpyAsync(h->h_counts + 3 * MB + 4, h->d_err, sizeof(int) * 4, cudaMemcpyDeviceToHost, st));
     ORB_CUDA(cudaEventRecord(r->ev_counts, st));
     r->pending = true;
-    r->n_frames = nf; r->nq_last = QL ? nqL : -1; r->nq_local = (QC || CH) ? nqC : -1; r->with_po = po ? 1 : 0; r->chain_np = CH ? nqC : -1;
+    r->n_frames = nf; r->nimg = nimg; r->mono = mono;
+    r->nq_last = QL ? nqL : -1; r->nq_local = (QC || CH) ? nqC : -1; r->with_po = po ? 1 : 0; r->chain_np = CH ? nqC : -1;
     return ORB_OK;
 }
 
@@ -313,7 +322,7 @@ extern "C" orb_status orbr_collect(orbx_handle* h, const orbr_results* O, int32_
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     ORB_CUDA(cudaEventSynchronize(r->ev_counts));
     r->pending = false;
-    const int MB = h->cfg.max_batch, nimg = 2 * r->n_frames, nf = r->n_frames;
+    const int MB = h->cfg.max_batch, nimg = r->nimg, nf = r->n_frames;
     h->counts_valid = true;
     const int* e = h->h_counts + 3 * MB + 4;
     h->batch_status = (e[0] || e[1]) ? (e[0] ? 1 : 2) : 0;
@@ -332,8 +341,12 @@ extern "C" orb_status orbr_collect(orbx_handle* h, const orbr_results* O, int32_
         return ORB_OK;
     };
     orb_status s;
-    if ((s = down(O->keypoints, h->d_kps, sizeof(orbx_keypoint) * (size_t)rows)) != ORB_OK || (s = down(O->descriptors, h->d_desc, 32 * (size_t)rows)) != ORB_OK ||
-        (s = down(O->uright, h->d_uright, 4 * (size_t)rows)) != ORB_OK || (s = down(O->depth, h->d_depth, 4 * (size_t)rows)) != ORB_OK)
+    if ((s = down(O->keypoints, h->d_kps, sizeof(orbx_keypoint) * (size_t)rows)) != ORB_OK || (s = down(O->descriptors, h->d_desc, 32 * (size_t)rows)) != ORB_OK)
+        return s;
+    if (r->mono) {   // the monocular Frame stores mvuRight = mvDepth = -1; d_uright may still hold an earlier stereo batch
+        if (O->uright) std::fill(O->uright, O->uright + rows, -1.0f);
+        if (O->depth) std::fill(O->depth, O->depth + rows, -1.0f);
+    } else if ((s = down(O->uright, h->d_uright, 4 * (size_t)rows)) != ORB_OK || (s = down(O->depth, h->d_depth, 4 * (size_t)rows)) != ORB_OK)
         return s;
     if (r->nq_last >= 0) {
         if ((s = down(O->last_feature_match, r->d_fm, 4 * (size_t)rows)) != ORB_OK || (s = down(O->last_nmatches, r->d_nm_last, 4 * (size_t)nf)) != ORB_OK) return s;

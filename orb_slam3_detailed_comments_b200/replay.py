@@ -72,31 +72,34 @@ def max_over_ranks(ms, device):
 
 # ---- native replay step (include/orbslam3_b200.h: orbr_submit / orbr_collect) -----------------------------------------------
 class TrackingStep:
-    """The tracking-thread step of a batch of stereo frames on one extractor handle, host buffers in / host buffers out:
-    `submit` queues the image upload, both eyes' extraction, ComputeStereoMatches, SearchByProjection(cur, last),
+    """The tracking-thread step of a batch of stereo or monocular frames on one extractor handle, host buffers in / host buffers
+    out: `submit` queues the image upload, the extraction (both eyes, then ComputeStereoMatches; or with monocular=True one image
+    per frame with vLappingArea = {0, 1000} and mvuRight = -1, Frame.cc:380), SearchByProjection(cur, last),
     SearchByProjection(F, local map points) and (optionally) PoseOptimization after each search, and returns at once;
     `collect` waits and copies the results into the caller's (ideally pinned) arrays.  Keep several handles in flight from
-    one host thread: submit on handles k+1 .. k+H-1 before collecting handle k."""
+    one host thread: submit on handles k+1 .. k+H-1 before collecting handle k.  A monocular step takes direction 0 for every
+    frame (bMono) and ignores bf / b."""
 
     def __init__(self, extractor, cam, bf, b, th_last=15.0, th_local=3.0, nnratio_local=0.8, check_orientation=True, far_points=False,
-                 th_far=50.0):
+                 th_far=50.0, monocular=False):
         import ctypes as C
         from . import _native as N
         self._C, self._N, self._L = C, N, N.lib()
         self.ex, self.cam = extractor, cam
         self.args = (float(bf), float(b), float(th_last), 1 if check_orientation else 0, float(th_local), float(nnratio_local),
                      1 if far_points else 0, float(th_far))
+        self.monocular = bool(monocular)
         self._keep = None
 
     def submit(self, images, last=None, local=None, pose=None, local_world_pos=None, chain=None):
-        """images: (2 * n_frames, H, W) uint8 host array; last / local: dicts of host arrays with the field names of
+        """images: (2 * n_frames, H, W) uint8 host array, (n_frames, H, W) for a monocular step; last / local: dicts of host arrays with the field names of
         orbm_last_queries / orbm_local_queries (fimg, off, Tcw, dir, xw, oct, ang, desc, obs / fimg, off, px, py, pxr, lvl, vc, desc
         [, td, in_view]); pose + local_world_pos switch PoseOptimization on.  chain: dict(off, xw, normal, max_dist, min_dist, desc,
         last_query[, cos_limit]) of the frames' local map points selects the chained flow (orbr_chain): needs last and pose, no local."""
         C, N = self._C, self._N
         assert images.dtype == np.uint8 and images.flags["C_CONTIGUOUS"] and images.ndim == 3
         nimg, h, w = images.shape
-        nf = nimg // 2
+        nf = nimg if self.monocular else nimg // 2
         bf, b, thl, ori, thc, nnr, far, thfar = self.args
         ql = qc = None
         if last is not None:
@@ -113,12 +116,12 @@ class TrackingStep:
         st = N.orbr_step(nf, N.ptr(images), w, h, w, w * h, bf, b, C.pointer(ql) if ql is not None else None, thl, ori,
                          C.pointer(qc) if qc is not None else None, thc, nnr, far, thfar, 1 if po else 0,
                          N.ptr(pose) if po else None, N.ptr(local_world_pos) if (po and local_world_pos is not None) else None,
-                         C.pointer(ch) if ch is not None else None)
+                         C.pointer(ch) if ch is not None else None, 1 if self.monocular else 0)
         self._keep = (images, last, local, pose, local_world_pos, ql, qc, chain, ch)      # the arrays must outlive the asynchronous copies
         N.check(self._L.orbr_submit(self.ex._h, C.byref(self.cam), C.byref(st)))
 
     def collect(self, out):
-        """out: dict of preallocated host arrays -- kps, desc, ur, dep (cap_rows rows), n, offsets, fm, nm1, mt, nm2 and, with
+        """out: dict of preallocated host arrays -- kps, desc, ur, dep (cap_rows rows), n, offsets (one entry per image, + 1), fm, nm1, mt, nm2 and, with
         PoseOptimization, pose (2, nf, 7) f64, inl (2, nf) i32, eoff (2, nf + 1) i32, efeat (2, cap) i32, outl (2, cap) u8; chained
         flow: c_in_view, c_px, c_py, c_pxr, c_level, c_vc (per local map point) and c_pose (nf, 7) f32.
         Missing keys are not copied back.  Returns the number of compact rows of the batch."""
