@@ -413,7 +413,12 @@ extern "C" orb_status orbo_pose_edges(orbx_handle* h, const orbo_edge_source* sr
     const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, [&](Carve& c) { P.cnt = c.take<int>(nf); });
     if (s != ORB_OK) return s;
     P.eoff = edge_offset_out; P.efeat = edge_feature_out; P.exw = world_pos_out; P.eobs = obs_out; P.ew = inv_sigma2_out;
+    // one int per row of the handle: past 12 276 rows (48 KB less the 48 B of static arrays) the launch needs more than the default
+    // window.  It always fits the opt-in limit: a handle has extracted a batch (checked above), and extraction refuses any row capacity
+    // whose k_order block ((rows + 64) x 4 B plus its static arrays, extractor.cu) does not fit, which is the larger of the two
     const size_t sm = (size_t)P.maxFeat * 4;
+    ORB_CUDA(cudaFuncSetAttribute(k_pose_edges<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    ORB_CUDA(cudaFuncSetAttribute(k_pose_edges<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
     k_pose_edges<false><<<nf, PE_THREADS, sm, h->stream>>>(P, nf);
     ORB_LAUNCHED();
     k_pose_edges<true><<<nf, PE_THREADS, sm, h->stream>>>(P, nf);
