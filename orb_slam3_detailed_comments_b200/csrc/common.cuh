@@ -64,18 +64,41 @@ inline int device_sm_count(int device) {
     return n > 0 ? n : 1;
 }
 
+// One thread-block cluster of `cs` CTAs per problem (solvers k_lba, k_liba): one or two problems get 16 CTAs each (the non-portable
+// cluster size), larger batches 8, 4 or 2 while all their clusters fit the SMs at once, then one CTA each.
+inline int cluster_size_for(int n_problems, int sms) {
+    if (n_problems <= 2) return 16;
+    int cs = 8;
+    while (cs > 1 && n_problems * cs > sms) cs >>= 1;
+    return cs;
+}
+
+inline void cluster_config(cudaLaunchConfig_t& cfg, cudaLaunchAttribute& at, int grid, int cs, int threads, size_t smem, cudaStream_t st) {
+    cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    at.id = cudaLaunchAttributeClusterDimension;
+    at.val.clusterDim.x = cs; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+    cfg.attrs = &at; cfg.numAttrs = 1;
+}
+
+// n_problems clusters of cs CTAs; the CTAs of a problem are consecutive in x
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_cluster(void (*kern)(KArgs...), int n_problems, int cs, int threads, size_t smem, cudaStream_t st, Args&&... args) {
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute at;
+    cluster_config(cfg, at, n_problems * cs, cs, threads, smem, st);
+    return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+}
+
 // Halve a thread-block cluster size (*cs) until the device can co-schedule one cluster of `kern` with this block and dynamic shared
 // memory: a 16-CTA (non-portable) cluster needs 16 SMs with room for the block inside one GPC, which not every H100 GPC has.  A
 // failing query is returned as the error it is, never taken for "does not fit".
 template <typename... KArgs>
 inline cudaError_t fit_cluster_size(void (*kern)(KArgs...), int* cs, int threads, size_t smem) {
     while (*cs > 1) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(*cs); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = *cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
+        cudaLaunchConfig_t cfg;
+        cudaLaunchAttribute at;
+        cluster_config(cfg, at, *cs, *cs, threads, smem, nullptr);
         int n = 0;
         const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
         if (e != cudaSuccess) return e;

@@ -26,6 +26,7 @@
 
 #include "common.cuh"
 #include "ba_math.cuh"
+#include "lba_pack.h"
 #include "scratch.h"
 
 using namespace orb;
@@ -34,65 +35,6 @@ namespace orb {
 
 #define LBA_THREADS 256
 #define LBA_CS_MAX 16    // CTAs (SMs) per problem: 16 (the non-portable cluster size sm_90 allows) for one or two problems, 8 while they fit the SMs
-#define LBA_ICH 128      // co-observation items per Schur task
-#define LBA_SMEM_N 144   // reduced systems up to 144 x 144 (24 free keyframes) are factorised in shared memory
-
-struct LbaDev {
-    int nKF, nMP, nE, nP, n;   // n = 6 * nP
-    // inputs
-    const double* pose0;   // [nKF][7] qx qy qz qw tx ty tz
-    const double* point0;  // [nMP][3]
-    const int* pidx;       // [nKF] pose index or -1 (fixed)
-    const int* ekf;
-    const int* emp;
-    const double* obs;     // [nE][3], ur < 0 => monocular edge
-    const double* invs2;
-    const int* mpStart;    // [nMP + 1]
-    const int* mpEdge;     // edges grouped by map point
-    const int* poseStart;  // [nP + 1]
-    const int* poseEdge;   // edges grouped by free pose
-    const int* pairStart;  // [nPairBlocks + 1]: item slots of pose-block pair b are [pairStart[b], pairStart[b+1])
-    const int* ptItemStart;  // [nMP + 1]: items generated by landmark l
-    const int4* ptItem;      // (e1, e2, slot, 0): same landmark, pose(e1) <= pose(e2); slot = position inside its block pair
-    int nItems, nTasks, nFreeEdges;
-    const int* taskStart;   // [nTasks + 1] item ranges (<= LBA_ICH items, never across a pose-block pair)
-    const int* blockTask;   // [nPairBlocks + 1] tasks of every pose-block pair
-    double* taskSum;        // [nTasks][36]
-    double* BD;             // [nE][18] B_e D_l^-1
-    const int* poseSlot;     // [nE] position of the edge in the pose-sorted order (-1: fixed pose)
-    const int* blockP1;    // [nPairBlocks]
-    const int* blockP2;
-    int nPairBlocks;
-    double fx, fy, cx, cy, bf, lambdaInit;
-    int maxIters;
-    const volatile int* stop;   // mapped host flag or null
-    // state + scratch
-    double* pose;     // current estimate
-    double* point;
-    double* poseSave;
-    double* pointSave;
-    double* Hpl;      // [nE][18]
-    double* W;        // [pose-sorted slot][27] per-edge pose terms (21 upper H + 6 b)
-    double* Prod;     // [item slot][36] B_e1 D^-1 B_e2^T of every co-observation pair
-    double* Hll;      // [nMP][9]
-    double* bl;       // [nMP][3]
-    double* Dinv;     // [nMP][9]
-    double* db;       // [nMP][3]
-    double* Hpp;      // [nP][36]
-    double* bp;       // [nP][6]
-    double* xl;       // [nMP][3]
-    double* HsGlobal; // [n][n] when n > LBA_SMEM_N
-    double* posePart; // [nP * LBA_PCH][27] partial pose sums
-    double* HsBlocks; // [nPairBlocks][36] Schur sums per pose-block pair
-    double* bs;       // [n] reduced right-hand side
-    double* xp;       // [n] pose update
-    double* partials; // [LBA_CS_MAX] cross-CTA reduction scratch
-    int* flags;       // [0] / [2] stop requested (alternating), [1] factorisation ok
-    double* err;      // [nE] chi2 per edge (last evaluation)
-    // outputs
-    uint8_t* depthPos;   // [nE]
-    double* stats;       // iterations, lambda, chi2, trials, initial chi2
-};
 
 __device__ __forceinline__ int edge_error(const LbaDev& P, int e, double r[3], double Xc[3]) {
     se3_map(P.pose + 7 * P.ekf[e], P.point + 3 * P.emp[e], Xc);
@@ -265,7 +207,6 @@ __device__ void build_points(const LbaDev& P, const Huber& H, int gtid, int gstr
 // B phase, part 2: H_pp / b_p = per-pose sums of the per-edge terms.  The terms are stored in pose-sorted order,
 // so a warp streams a contiguous [slots][27] slab (lane = term).  Each pose is cut into LBA_PCH chunks handled by
 // different warps of the team; partial sums are combined in a fixed order (deterministic).
-#define LBA_PCH 8
 __device__ void build_poses(const LbaDev& P, const Team& T) {
     const int lane = T.tid & 31;
     for (int task = T.gwarp; task < P.nP * LBA_PCH; task += T.nwarps) {
@@ -752,156 +693,34 @@ __global__ void __launch_bounds__(LBA_THREADS, 1) k_lba(const LbaDev* __restrict
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-struct lba_handle {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    uint8_t* d_buf = nullptr;
-    size_t d_bytes = 0;
-    uint8_t* h_buf = nullptr;      // pinned staging
-    size_t h_bytes = 0;
+struct lba_handle : SolverHandle {
     int* h_stop = nullptr;         // mapped pinned flag the kernel polls
     int* d_stop = nullptr;
-    int n_sms = 1;
 };
 
-extern "C" orb_status lba_create(int32_t device, lba_handle** out) {
-    if (!out) return set_error(ORB_ERR_INVALID, "null argument");
-    *out = nullptr;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
-        return set_error(ORB_ERR_NO_DEVICE, "no usable CUDA device (this library has no CPU fallback)");
-    ORB_CUDA(cudaSetDevice(device));
-    lba_handle* h = new lba_handle();
-    h->device = device;
-    h->n_sms = device_sm_count(device);
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
-        delete h;
-        return set_error(ORB_ERR_CUDA, "cudaStreamCreate failed");
-    }
-    if (cudaHostAlloc((void**)&h->h_stop, sizeof(int), cudaHostAllocMapped) != cudaSuccess ||
-        cudaHostGetDevicePointer((void**)&h->d_stop, h->h_stop, 0) != cudaSuccess) {
-        cudaStreamDestroy(h->stream);
-        delete h;
-        return set_error(ORB_ERR_CUDA, "mapped stop flag allocation failed");
-    }
-    *h->h_stop = 0;
-    ORB_CUDA(cudaFuncSetAttribute(k_lba, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    ORB_CUDA(cudaFuncSetAttribute(k_lba, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)((LBA_THREADS + 960 + 12 * LBA_SMEM_N + 8 + LBA_SMEM_N * LBA_SMEM_N) * sizeof(double))));
-    *out = h;
-    return ORB_OK;
-}
+// k_lba's dynamic shared memory with a reduced system of n x n in it
+static size_t lba_smem_bytes(int n) { return (LBA_THREADS + 960 + 12 * LBA_SMEM_N + 8 + (size_t)n * n) * sizeof(double); }
 
 extern "C" void lba_destroy(lba_handle* h) {
     if (!h) return;
-    cudaSetDevice(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    if (h->d_buf) cudaFree(h->d_buf);
-    if (h->h_buf) cudaFreeHost(h->h_buf);
+    solver_release(h);
     if (h->h_stop) cudaFreeHost(h->h_stop);
-    if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
 
-namespace {
-struct Carver {
-    size_t off = 0;
-    size_t take(size_t bytes) {
-        off = (off + 255) / 256 * 256;
-        const size_t o = off;
-        off += bytes;
-        return o;
+extern "C" orb_status lba_create(int32_t device, lba_handle** out) {
+    const orb_status s = solver_create(device, k_lba, lba_smem_bytes(LBA_SMEM_N), out);
+    if (s != ORB_OK) return s;
+    lba_handle* h = *out;
+    if (cudaHostAlloc((void**)&h->h_stop, sizeof(int), cudaHostAllocMapped) != cudaSuccess ||
+        cudaHostGetDevicePointer((void**)&h->d_stop, h->h_stop, 0) != cudaSuccess) {
+        lba_destroy(h);
+        *out = nullptr;
+        return set_error(ORB_ERR_CUDA, "mapped stop flag allocation failed");
     }
-};
-
-struct Prep {   // host-side index structures of one problem (offsets into the staging buffer)
-    int nP = 0, nBlocks = 0;
-    std::vector<int> pidx, mpStart, mpEdge, poseStart, poseEdge, pairStart, blockP1, blockP2, ptItemStart, poseSlot;
-    std::vector<int4> ptItem;
-    std::vector<int> taskStart, blockTask;
-};
-
-orb_status prepare(const lba_problem& in, Prep& R) {
-    const int nKF = in.n_kf, nMP = in.n_mp, nE = in.n_edges;
-    R.pidx.assign(nKF, -1);
-    R.nP = 0;
-    for (int k = 0; k < nKF; ++k)
-        if (!in.fixed[k]) R.pidx[k] = R.nP++;
-    if (R.nP > 160) return set_error(ORB_ERR_UNSUPPORTED, "more than 160 free keyframes in one local BA");
-    R.mpStart.assign(nMP + 1, 0);
-    R.poseStart.assign(R.nP + 1, 0);
-    for (int e = 0; e < nE; ++e) {
-        if (in.edge_kf[e] < 0 || in.edge_kf[e] >= nKF || in.edge_mp[e] < 0 || in.edge_mp[e] >= nMP)
-            return set_error(ORB_ERR_INVALID, "edge index out of range");
-        ++R.mpStart[in.edge_mp[e] + 1];
-        const int p = R.pidx[in.edge_kf[e]];
-        if (p >= 0) ++R.poseStart[p + 1];
-    }
-    for (int l = 0; l < nMP; ++l) R.mpStart[l + 1] += R.mpStart[l];
-    for (int p = 0; p < R.nP; ++p) R.poseStart[p + 1] += R.poseStart[p];
-    R.mpEdge.resize(nE);
-    R.poseEdge.resize(R.poseStart[R.nP]);
-    {
-        std::vector<int> a(R.mpStart.begin(), R.mpStart.end() - 1), b(R.poseStart.begin(), R.poseStart.end() - 1);
-        for (int e = 0; e < nE; ++e) {
-            R.mpEdge[a[in.edge_mp[e]]++] = e;
-            const int p = R.pidx[in.edge_kf[e]];
-            if (p >= 0) R.poseEdge[b[p]++] = e;
-        }
-    }
-    // upper pose-block pairs that share at least one landmark (the sparsity pattern of H_schur,
-    // block_solver.hpp:199-238) + every diagonal block
-    const int nP = R.nP;
-    std::vector<int> cnt((size_t)nP * nP, 0);
-    for (int l = 0; l < nMP; ++l)
-        for (int a = R.mpStart[l]; a < R.mpStart[l + 1]; ++a) {
-            const int p1 = R.pidx[in.edge_kf[R.mpEdge[a]]];
-            if (p1 < 0) continue;
-            for (int b = R.mpStart[l]; b < R.mpStart[l + 1]; ++b) {
-                const int p2 = R.pidx[in.edge_kf[R.mpEdge[b]]];
-                if (p2 < p1) continue;
-                if (p2 == p1 && b != a) continue;   // a landmark has one edge per keyframe; guard duplicates
-                ++cnt[(size_t)p1 * nP + p2];
-            }
-        }
-    std::vector<int> blockOf((size_t)nP * nP, -1);
-    R.blockP1.clear(); R.blockP2.clear(); R.pairStart.assign(1, 0);
-    for (int p1 = 0; p1 < nP; ++p1)
-        for (int p2 = p1; p2 < nP; ++p2)
-            if (cnt[(size_t)p1 * nP + p2] > 0 || p1 == p2) {
-                blockOf[(size_t)p1 * nP + p2] = (int)R.blockP1.size();
-                R.blockP1.push_back(p1);
-                R.blockP2.push_back(p2);
-                R.pairStart.push_back(R.pairStart.back() + cnt[(size_t)p1 * nP + p2]);
-            }
-    R.nBlocks = (int)R.blockP1.size();
-    R.ptItem.assign(R.pairStart.back(), make_int4(0, 0, 0, 0));   // items stored block by block
-    R.ptItemStart.assign(nMP + 1, 0);
-    std::vector<int> fill(R.pairStart.begin(), R.pairStart.end() - 1);
-    for (int l = 0; l < nMP; ++l) {
-        for (int a = R.mpStart[l]; a < R.mpStart[l + 1]; ++a) {
-            const int e1 = R.mpEdge[a], p1 = R.pidx[in.edge_kf[e1]];
-            if (p1 < 0) continue;
-            for (int b = R.mpStart[l]; b < R.mpStart[l + 1]; ++b) {
-                const int e2 = R.mpEdge[b], p2 = R.pidx[in.edge_kf[e2]];
-                if (p2 < p1) continue;
-                if (p2 == p1 && b != a) continue;
-                R.ptItem[fill[blockOf[(size_t)p1 * nP + p2]]++] = make_int4(e1, e2, 0, l);
-            }
-        }
-        R.ptItemStart[l + 1] = 0;   // (per-landmark item lists are no longer used)
-    }
-    R.taskStart.assign(1, 0);
-    R.blockTask.assign(1, 0);
-    for (int b = 0; b < R.nBlocks; ++b) {
-        for (int k = R.pairStart[b]; k < R.pairStart[b + 1]; k += LBA_ICH) R.taskStart.push_back(std::min(k + LBA_ICH, R.pairStart[b + 1]));
-        R.blockTask.push_back((int)R.taskStart.size() - 1);
-    }
-    R.poseSlot.assign(nE, -1);
-    for (int k = 0; k < (int)R.poseEdge.size(); ++k) R.poseSlot[R.poseEdge[k]] = k;
+    *h->h_stop = 0;
     return ORB_OK;
 }
-}  // namespace
 
 // *pbStopFlag of the reference is a C++ bool written by another thread (LocalMapping::InterruptBA); the C ABI also takes an
 // int32 flag.  flag_bytes selects how the relay reads it.
@@ -913,128 +732,36 @@ static orb_status lba_solve_impl(lba_handle* h, int32_t n_problems, const lba_pr
                                  int flag_bytes) {
     if (!h || !in || !out || n_problems < 1) return set_error(ORB_ERR_INVALID, "bad arguments");
     ORB_CUDA(cudaSetDevice(h->device));
-    std::vector<Prep> prep(n_problems);
-    std::vector<LbaDev> dev(n_problems);
-    // pass 1: sizes.  Every array lives in one device buffer; inputs are staged in one pinned buffer with the
-    // same offsets so a single H2D moves them all.
-    Carver in_c, work_c;
-    struct Offs { size_t pose0, point0, pidx, ekf, emp, obs, invs2, mpStart, mpEdge, poseStart, poseEdge, pairStart, ptItemStart, ptItem, poseSlot, bP1, bP2, taskStart, blockTask;
-                  size_t pose, point, poseS, pointS, Hpl, W, Prod, posePart, HsBlocks, bs, xp, partials, flags, taskSum, BD, Hll, bl, Dinv, db, Hpp, bp, xl, Hs, err, dpos, stats; };
-    std::vector<Offs> offs(n_problems);
+    std::vector<LbaPrep> prep(n_problems);
     for (int i = 0; i < n_problems; ++i) {
         const lba_problem& p = in[i];
         if (p.n_kf < 1 || p.n_mp < 1 || p.n_edges < 1 || !p.pose || !p.fixed || !p.point || !p.edge_kf || !p.edge_mp || !p.obs ||
             !p.inv_sigma2 || !out[i].pose || !out[i].point)
             return set_error(ORB_ERR_INVALID, "incomplete lba_problem / lba_result");
-        orb_status s = prepare(p, prep[i]);
-        if (s != ORB_OK) return s;
-        const Prep& R = prep[i];
-        Offs& o = offs[i];
-        const size_t nKF = p.n_kf, nMP = p.n_mp, nE = p.n_edges, nP = R.nP, n = 6 * nP;
-        o.pose0 = in_c.take(nKF * 56); o.point0 = in_c.take(nMP * 24); o.pidx = in_c.take(nKF * 4);
-        o.ekf = in_c.take(nE * 4); o.emp = in_c.take(nE * 4); o.obs = in_c.take(nE * 24); o.invs2 = in_c.take(nE * 8);
-        o.mpStart = in_c.take((nMP + 1) * 4); o.mpEdge = in_c.take(nE * 4);
-        o.poseStart = in_c.take((nP + 1) * 4); o.poseEdge = in_c.take(R.poseEdge.size() * 4 + 4);
-        o.pairStart = in_c.take((R.nBlocks + 1) * 4); o.ptItemStart = in_c.take((nMP + 1) * 4);
-        o.ptItem = in_c.take(R.ptItem.size() * 16 + 16); o.poseSlot = in_c.take(nE * 4);
-        o.taskStart = in_c.take(R.taskStart.size() * 4); o.blockTask = in_c.take(R.blockTask.size() * 4);
-        o.bP1 = in_c.take(R.nBlocks * 4 + 4); o.bP2 = in_c.take(R.nBlocks * 4 + 4);
-        o.pose = work_c.take(nKF * 56); o.point = work_c.take(nMP * 24); o.poseS = work_c.take(nKF * 56); o.pointS = work_c.take(nMP * 24);
-        o.Hpl = work_c.take(nE * 144); o.W = work_c.take(R.poseEdge.size() * 216 + 216);
-        o.Prod = work_c.take(288); o.posePart = work_c.take(nP * 8 * 216 + 216);
-        o.HsBlocks = work_c.take((size_t)R.nBlocks * 288 + 288); o.bs = work_c.take(n * 8 + 8); o.xp = work_c.take(n * 8 + 8);
-        o.partials = work_c.take(64 * 8); o.flags = work_c.take(64);
-        o.taskSum = work_c.take(R.taskStart.size() * 288 + 288); o.BD = work_c.take(nE * 144 + 144); o.Hll = work_c.take(nMP * 72); o.bl = work_c.take(nMP * 24);
-        o.Dinv = work_c.take(nMP * 72); o.db = work_c.take(nMP * 24); o.Hpp = work_c.take(nP * 288 + 8); o.bp = work_c.take(nP * 48 + 8);
-        o.xl = work_c.take(nMP * 24); o.Hs = work_c.take(n > LBA_SMEM_N ? n * n * 8 : 8); o.err = work_c.take(nE * 8);
-        o.dpos = work_c.take(nE); o.stats = work_c.take(256);
+        const char* why = nullptr;
+        const orb_status s = lba_prepare(p, prep[i], &why);
+        if (s != ORB_OK) return set_error(s, why);
     }
-    const size_t in_bytes = (in_c.off + 255) / 256 * 256, work_bytes = work_c.off + 256;
-    const size_t desc_off = in_bytes, desc_bytes = (sizeof(LbaDev) * n_problems + 255) / 256 * 256;
-    orb_status s = grow_device(h->d_bytes, h->d_buf, in_bytes + desc_bytes + work_bytes, false);
-    if (s != ORB_OK || (s = grow_pinned(h->h_bytes, h->h_buf, in_bytes + desc_bytes)) != ORB_OK) return s;
+    const volatile int* stop = stop_flag ? h->d_stop : nullptr;
+    const LbaLayout lay = lba_pack(n_problems, in, prep.data(), stop, nullptr, nullptr);
+    const size_t mirror = lay.in_bytes + lay.desc_bytes;
+    orb_status s = grow_device(h->d_bytes, h->d_buf, mirror + lay.work_bytes, false);
+    if (s != ORB_OK || (s = grow_pinned(h->h_bytes, h->h_buf, mirror)) != ORB_OK) return s;
     uint8_t* hb = h->h_buf;
-    uint8_t* db = h->d_buf;
-    uint8_t* dwork = db + in_bytes + desc_bytes;
-    for (int i = 0; i < n_problems; ++i) {
-        const lba_problem& p = in[i];
-        const Prep& R = prep[i];
-        const Offs& o = offs[i];
-        memcpy(hb + o.pose0, p.pose, (size_t)p.n_kf * 56);
-        memcpy(hb + o.point0, p.point, (size_t)p.n_mp * 24);
-        memcpy(hb + o.pidx, R.pidx.data(), (size_t)p.n_kf * 4);
-        memcpy(hb + o.ekf, p.edge_kf, (size_t)p.n_edges * 4);
-        memcpy(hb + o.emp, p.edge_mp, (size_t)p.n_edges * 4);
-        memcpy(hb + o.obs, p.obs, (size_t)p.n_edges * 24);
-        memcpy(hb + o.invs2, p.inv_sigma2, (size_t)p.n_edges * 8);
-        memcpy(hb + o.mpStart, R.mpStart.data(), R.mpStart.size() * 4);
-        memcpy(hb + o.mpEdge, R.mpEdge.data(), R.mpEdge.size() * 4);
-        memcpy(hb + o.poseStart, R.poseStart.data(), R.poseStart.size() * 4);
-        if (!R.poseEdge.empty()) memcpy(hb + o.poseEdge, R.poseEdge.data(), R.poseEdge.size() * 4);
-        memcpy(hb + o.pairStart, R.pairStart.data(), R.pairStart.size() * 4);
-        memcpy(hb + o.ptItemStart, R.ptItemStart.data(), R.ptItemStart.size() * 4);
-        if (!R.ptItem.empty()) memcpy(hb + o.ptItem, R.ptItem.data(), R.ptItem.size() * 16);
-        memcpy(hb + o.poseSlot, R.poseSlot.data(), R.poseSlot.size() * 4);
-        memcpy(hb + o.taskStart, R.taskStart.data(), R.taskStart.size() * 4);
-        memcpy(hb + o.blockTask, R.blockTask.data(), R.blockTask.size() * 4);
-        if (R.nBlocks) {
-            memcpy(hb + o.bP1, R.blockP1.data(), (size_t)R.nBlocks * 4);
-            memcpy(hb + o.bP2, R.blockP2.data(), (size_t)R.nBlocks * 4);
-        }
-        LbaDev& D = dev[i];
-        D.nKF = p.n_kf; D.nMP = p.n_mp; D.nE = p.n_edges; D.nP = R.nP; D.n = 6 * R.nP;
-        D.pose0 = (const double*)(db + o.pose0); D.point0 = (const double*)(db + o.point0); D.pidx = (const int*)(db + o.pidx);
-        D.ekf = (const int*)(db + o.ekf); D.emp = (const int*)(db + o.emp); D.obs = (const double*)(db + o.obs);
-        D.invs2 = (const double*)(db + o.invs2); D.mpStart = (const int*)(db + o.mpStart); D.mpEdge = (const int*)(db + o.mpEdge);
-        D.poseStart = (const int*)(db + o.poseStart); D.poseEdge = (const int*)(db + o.poseEdge);
-        D.pairStart = (const int*)(db + o.pairStart); D.ptItemStart = (const int*)(db + o.ptItemStart);
-        D.ptItem = (const int4*)(db + o.ptItem); D.poseSlot = (const int*)(db + o.poseSlot);
-        D.nFreeEdges = (int)R.poseEdge.size();
-        D.nItems = (int)R.ptItem.size(); D.nTasks = (int)R.taskStart.size() - 1;
-        D.taskStart = (const int*)(db + o.taskStart); D.blockTask = (const int*)(db + o.blockTask);
-        D.blockP1 = (const int*)(db + o.bP1); D.blockP2 = (const int*)(db + o.bP2); D.nPairBlocks = R.nBlocks;
-        D.fx = p.fx; D.fy = p.fy; D.cx = p.cx; D.cy = p.cy; D.bf = p.bf; D.lambdaInit = p.lambda_init; D.maxIters = p.max_iters;
-        D.stop = stop_flag ? h->d_stop : nullptr;
-        D.pose = (double*)(dwork + o.pose); D.point = (double*)(dwork + o.point); D.poseSave = (double*)(dwork + o.poseS);
-        D.pointSave = (double*)(dwork + o.pointS); D.Hpl = (double*)(dwork + o.Hpl); D.W = (double*)(dwork + o.W);
-        D.Prod = (double*)(dwork + o.Prod); D.posePart = (double*)(dwork + o.posePart);
-        D.HsBlocks = (double*)(dwork + o.HsBlocks); D.bs = (double*)(dwork + o.bs); D.xp = (double*)(dwork + o.xp);
-        D.partials = (double*)(dwork + o.partials); D.flags = (int*)(dwork + o.flags);
-        D.taskSum = (double*)(dwork + o.taskSum); D.BD = (double*)(dwork + o.BD);
-        D.Hll = (double*)(dwork + o.Hll); D.bl = (double*)(dwork + o.bl); D.Dinv = (double*)(dwork + o.Dinv); D.db = (double*)(dwork + o.db);
-        D.Hpp = (double*)(dwork + o.Hpp); D.bp = (double*)(dwork + o.bp); D.xl = (double*)(dwork + o.xl); D.HsGlobal = (double*)(dwork + o.Hs);
-        D.err = (double*)(dwork + o.err); D.depthPos = dwork + o.dpos; D.stats = (double*)(dwork + o.stats);
-    }
-    memcpy(hb + desc_off, dev.data(), sizeof(LbaDev) * n_problems);
+    lba_pack(n_problems, in, prep.data(), stop, hb, h->d_buf);
+    const LbaDev* dev = reinterpret_cast<const LbaDev*>(hb + lay.in_bytes);
     *h->h_stop = (stop_flag && read_stop_flag(stop_flag, flag_bytes)) ? 1 : 0;
-    ORB_CUDA(cudaMemcpyAsync(db, hb, in_bytes + desc_bytes, cudaMemcpyHostToDevice, h->stream));
+    ORB_CUDA(cudaMemcpyAsync(h->d_buf, hb, mirror, cudaMemcpyHostToDevice, h->stream));
     // k_lba keeps a problem's reduced system in shared memory iff ITS n <= LBA_SMEM_N, so the launch must carry the largest such
     // n -- not the batch-wide maximum: a batch mixing a > 24-keyframe problem with smaller ones still needs the smaller ones' slots
     int maxn = 0;
     for (int i = 0; i < n_problems; ++i)
         if (dev[i].n <= LBA_SMEM_N) maxn = std::max(maxn, dev[i].n);
-    const size_t smem = (LBA_THREADS + 960 + 12 * LBA_SMEM_N + 8 + (size_t)maxn * maxn) * sizeof(double);
-    // one thread-block cluster per problem; small batches get 8 SMs each, large batches fall back to one CTA each
-    const int sms = h->n_sms;
-    int cs = n_problems <= 2 ? 16 : (n_problems * 8 <= sms ? 8 : (n_problems * 4 <= sms ? 4 : (n_problems * 2 <= sms ? 2 : 1)));
+    const size_t smem = lba_smem_bytes(maxn);
+    int cs = cluster_size_for(n_problems, h->n_sms);
     if (const char* v = getenv("ORB_LBA_CLUSTER")) cs = std::max(1, std::min(atoi(v), cs));   // experiments: cap the cluster size
     ORB_CUDA(fit_cluster_size(k_lba, &cs, LBA_THREADS, smem));
-    {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(n_problems * cs);
-        cfg.blockDim = dim3(LBA_THREADS);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = h->stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = cs;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        const LbaDev* dptr = (const LbaDev*)(db + desc_off);
-        ORB_CUDA(cudaLaunchKernelEx(&cfg, k_lba, dptr, cs));
-    }
+    ORB_CUDA(launch_cluster(k_lba, n_problems, cs, LBA_THREADS, smem, h->stream, reinterpret_cast<const LbaDev*>(h->d_buf + lay.in_bytes), cs));
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
     // relay *pbStopFlag to the mapped flag while the kernel runs (LocalMapping::InterruptBA writes it asynchronously)
@@ -1047,13 +774,13 @@ static orb_status lba_solve_impl(lba_handle* h, int32_t n_problems, const lba_pr
     ORB_CUDA(cudaStreamSynchronize(h->stream));
     for (int i = 0; i < n_problems; ++i) {
         const lba_problem& p = in[i];
-        const Offs& o = offs[i];
-        ORB_CUDA(cudaMemcpyAsync(out[i].pose, dwork + o.pose, (size_t)p.n_kf * 56, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaMemcpyAsync(out[i].point, dwork + o.point, (size_t)p.n_mp * 24, cudaMemcpyDeviceToHost, h->stream));
-        if (out[i].edge_chi2) ORB_CUDA(cudaMemcpyAsync(out[i].edge_chi2, dwork + o.err, (size_t)p.n_edges * 8, cudaMemcpyDeviceToHost, h->stream));
+        const LbaDev& d = dev[i];
+        ORB_CUDA(cudaMemcpyAsync(out[i].pose, d.pose, (size_t)p.n_kf * 56, cudaMemcpyDeviceToHost, h->stream));
+        ORB_CUDA(cudaMemcpyAsync(out[i].point, d.point, (size_t)p.n_mp * 24, cudaMemcpyDeviceToHost, h->stream));
+        if (out[i].edge_chi2) ORB_CUDA(cudaMemcpyAsync(out[i].edge_chi2, d.err, (size_t)p.n_edges * 8, cudaMemcpyDeviceToHost, h->stream));
         if (out[i].edge_depth_positive)
-            ORB_CUDA(cudaMemcpyAsync(out[i].edge_depth_positive, dwork + o.dpos, (size_t)p.n_edges, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaMemcpyAsync(hb + 256 * i, dwork + o.stats, 160, cudaMemcpyDeviceToHost, h->stream));
+            ORB_CUDA(cudaMemcpyAsync(out[i].edge_depth_positive, d.depthPos, (size_t)p.n_edges, cudaMemcpyDeviceToHost, h->stream));
+        ORB_CUDA(cudaMemcpyAsync(hb + 256 * i, d.stats, 160, cudaMemcpyDeviceToHost, h->stream));
     }
     ORB_CUDA(cudaStreamSynchronize(h->stream));
     for (int i = 0; i < n_problems; ++i) {

@@ -18,7 +18,7 @@ static_assert(sizeof(liba_problem) == 232 && sizeof(liba_result) == 80, "C ABI l
 namespace {
 
 constexpr int LIBA_THREADS = 256;
-constexpr int LIBA_CS_MAX = 8;       // CTAs (SMs) per window: a portable-size thread-block cluster
+// CTAs per window: cluster_size_for (common.cuh), or ORB_LIBA_CLUSTER
 
 // One team (a cluster of `cs` CTAs, or one CTA) per window; blocks of a cluster are consecutive in x.
 __global__ void __launch_bounds__(LIBA_THREADS) k_liba(const LibaDev* __restrict__ problems, int cs) {
@@ -36,42 +36,13 @@ __global__ void __launch_bounds__(LIBA_THREADS) k_liba(const LibaDev* __restrict
 
 }  // namespace
 
-struct liba_handle {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    uint8_t* d_buf = nullptr;
-    size_t d_bytes = 0;
-    uint8_t* h_buf = nullptr;
-    size_t h_bytes = 0;
-    int n_sms = 1;
-};
+struct liba_handle : SolverHandle {};
 
-extern "C" orb_status liba_create(int32_t device, liba_handle** out) {
-    if (!out) return set_error(ORB_ERR_INVALID, "null argument");
-    *out = nullptr;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
-        return set_error(ORB_ERR_NO_DEVICE, "no usable CUDA device (this library has no CPU fallback)");
-    ORB_CUDA(cudaSetDevice(device));
-    liba_handle* h = new liba_handle();
-    h->device = device;
-    h->n_sms = device_sm_count(device);
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
-        delete h;
-        return set_error(ORB_ERR_CUDA, "cudaStreamCreate failed");
-    }
-    ORB_CUDA(cudaFuncSetAttribute(k_liba, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));   // 16-CTA clusters for one or two windows
-    *out = h;
-    return ORB_OK;
-}
+extern "C" orb_status liba_create(int32_t device, liba_handle** out) { return solver_create(device, k_liba, 0, out); }
 
 extern "C" void liba_destroy(liba_handle* h) {
     if (!h) return;
-    cudaSetDevice(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    if (h->d_buf) cudaFree(h->d_buf);
-    if (h->h_buf) cudaFreeHost(h->h_buf);
-    if (h->stream) cudaStreamDestroy(h->stream);
+    solver_release(h);
     delete h;
 }
 
@@ -105,34 +76,21 @@ extern "C" orb_status liba_solve(liba_handle* h, int32_t n_problems, const liba_
     if (s != ORB_OK || (s = grow_pinned(h->h_bytes, h->h_buf, total)) != ORB_OK) return s;
     LibaDev* hdev = reinterpret_cast<LibaDev*>(h->h_buf);
     ORB_CUDA(cudaMemsetAsync(h->d_buf, 0, total, h->stream));
-    for (int i = 0; i < n_problems; ++i) liba_pack(in[i], h->h_buf + base[i], h->d_buf + base[i], &hdev[i]);
+    for (int i = 0; i < n_problems; ++i) {
+        memset(h->h_buf + base[i], 0, lay[i].io_bytes + lay[i].in_bytes);
+        liba_pack(in[i], h->h_buf + base[i], h->d_buf + base[i], &hdev[i]);
+    }
     ORB_CUDA(cudaMemcpyAsync(h->d_buf, h->h_buf, sizeof(LibaDev) * (size_t)n_problems, cudaMemcpyHostToDevice, h->stream));
     for (int i = 0; i < n_problems; ++i)
         ORB_CUDA(cudaMemcpyAsync(h->d_buf + base[i], h->h_buf + base[i], lay[i].io_bytes + lay[i].in_bytes, cudaMemcpyHostToDevice, h->stream));
-    // one or two windows get a cluster of 16 SMs each (the non-portable size), small batches 8, large ones fewer
-    // (ORB_LIBA_CLUSTER = 1 | 2 | 4 | 8 | 16 overrides: a tuning knob)
-    const int sms = h->n_sms;
-    int cs = n_problems <= 2 ? 16 : ((n_problems * LIBA_CS_MAX <= sms) ? LIBA_CS_MAX : (n_problems * 4 <= sms ? 4 : (n_problems * 2 <= sms ? 2 : 1)));
+    // ORB_LIBA_CLUSTER = 1 | 2 | 4 | 8 | 16 overrides the cluster size: a tuning knob
+    int cs = cluster_size_for(n_problems, h->n_sms);
     if (const char* e = getenv("ORB_LIBA_CLUSTER")) {
         const int v = atoi(e);
         if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) cs = v;
     }
     ORB_CUDA(fit_cluster_size(k_liba, &cs, LIBA_THREADS, 0));
-    {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(n_problems * cs);
-        cfg.blockDim = dim3(LIBA_THREADS);
-        cfg.dynamicSmemBytes = 0;
-        cfg.stream = h->stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = cs;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        ORB_CUDA(cudaLaunchKernelEx(&cfg, k_liba, reinterpret_cast<const LibaDev*>(h->d_buf), cs));
-    }
+    ORB_CUDA(launch_cluster(k_liba, n_problems, cs, LIBA_THREADS, 0, h->stream, reinterpret_cast<const LibaDev*>(h->d_buf), cs));
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
     for (int i = 0; i < n_problems; ++i)

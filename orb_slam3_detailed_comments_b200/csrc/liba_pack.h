@@ -1,8 +1,9 @@
 // liba_pack.h -- host-side flattening of a liba_problem into one blob laid out for liba_core.cuh.  Pure host C++ so that the
 // CUDA wrapper (liba.cu) and the CPU emulation harness (tests/host_emul) share it.
 //   [io]   state, point, err, lerr, out_scalars, dpos            host -> device before, device -> host after
-//   [in]   obs, invs2, links, pidx, ekf, emp, pt_off, pt_edge
-//   [work] saved state, normal equations, Schur scratch    zero-filled
+//   [in]   obs, invs2, links, pidx, ekf, emp, the CSRs, co-observation lists    host -> device before
+//   [work] saved state, normal equations, Schur scratch    zero-filled on the device
+// The host range of io | in must be zero before the fill: its padding and the outputs in io are uploaded as they are.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -11,6 +12,7 @@
 
 #include "../../include/orbslam3_b200.h"
 #include "liba_core.cuh"
+#include "pack.h"
 
 namespace orb {
 
@@ -18,7 +20,7 @@ struct LibaLayout { size_t io_bytes = 0, in_bytes = 0, work_bytes = 0, total = 0
 
 static_assert(sizeof(liba_link) == 1080 && sizeof(LibaLink) == 1080, "liba_link layout");
 
-// host == nullptr: sizes only.  Pointers inside *dev are relative to devBase (== host for the CPU emulation).
+// devBase == nullptr: sizes only.  Pointers inside *dev are relative to devBase (== host for the CPU emulation).
 // Returns total == 0 when two links join the same keyframe pair (the gather in liba_build assumes at most one; the reference
 // creates one EdgeInertial per keyframe and its mPrevKF, Optimizer.cc:2430-2500).
 inline LibaLayout liba_pack(const liba_problem& p, uint8_t* host, uint8_t* devBase, LibaDev* dev) {
@@ -77,56 +79,34 @@ inline LibaLayout liba_pack(const liba_problem& p, uint8_t* host, uint8_t* devBa
         forEachCo([&](int pa, int pb, int e1, int e2) { const int q = pairIdx[(size_t)pa * nFree + pb]; coE1[cur[q]] = e1; coE2[cur[q]++] = e2; });
     }
 
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) & ~(size_t)15; return o; };
-    // io
-    const size_t oState = take(8 * 21 * (size_t)nKF), oPoint = take(8 * sl), oErr = take(8 * (size_t)nE), oLerr = take(8 * 3 * (size_t)nL), oOut = take(8 * 8), oDpos = take((size_t)nE);
-    lay.io_bytes = off;
-    // in
-    const size_t oObs = take(8 * 3 * (size_t)nE), oInv = take(8 * (size_t)nE), oLinks = take(sizeof(LibaLink) * (size_t)nL);
-    const size_t oPidx = take(4 * (size_t)nKF), oEkf = take(4 * (size_t)nE), oEmp = take(4 * (size_t)nE), oPtOff = take(4 * ((size_t)nMP + 1)), oPtEdge = take(4 * (size_t)nE),
-                 oKfOff = take(4 * ((size_t)nKF + 1)), oKfEdge = take(4 * (size_t)nE), oKlOff = take(4 * ((size_t)nKF + 1)), oKlEnt = take(4 * 2 * (size_t)nL),
-                 oPairP = take(4 * (size_t)nPairs), oPairOff = take(4 * ((size_t)nPairs + 1)), oCo1 = take(4 * nCo), oCo2 = take(4 * nCo);
-    lay.in_bytes = off - lay.io_bytes;
-    // work
-    const size_t oStateS = take(8 * 21 * (size_t)nKF), oPointS = take(8 * sl), oHpp = take(8 * sp * sp), oHs = take(8 * sp * sp), oB = take(8 * (sp + sl)), oBs = take(8 * sp),
-                 oX = take(8 * (sp + sl)), oY = take(8 * sp), oHll = take(8 * 9 * (size_t)nMP), oDinv = take(8 * 9 * (size_t)nMP), oW = take(8 * 18 * (size_t)nE),
-                 oWD = take(8 * 18 * (size_t)nE), oWdb = take(8 * 6 * (size_t)nE), oEpp = take(8 * 27 * (size_t)nE), oLblk = take(8 * 930 * (size_t)nL), oFlag = take(16), oPart = take(8 * 16),
-                 oChunk = take(8 * (size_t)LIBA_CHUNKS * std::max((size_t)27 * nKF, (size_t)36 * nPairs)), oChunkB = take(8 * (size_t)LIBA_CHUNKS * 6 * nKF), oYpan = take(8 * 15 * sp);
-    lay.work_bytes = off - lay.io_bytes - lay.in_bytes;
-    lay.total = off;
-    if (!host) return lay;
+    PackRegion r{devBase, host, 16};
+    LibaDev d;
+    d.state = r.put(p.state, 21 * (size_t)nKF); d.point = r.put(p.point, sl);
+    d.err = r.take<double>(nE); d.lerr = r.take<double>(3 * (size_t)nL); d.out_scalars = r.take<double>(8); d.dpos = r.take<uint8_t>(nE);
+    lay.io_bytes = r.bytes();
+    d.obs = r.put(p.obs, 3 * (size_t)nE); d.invs2 = r.put(p.inv_sigma2, nE); d.links = reinterpret_cast<const LibaLink*>(r.put(p.links, nL));
+    d.pidx = r.put(pidx.data(), nKF); d.ekf = r.put(p.edge_kf, nE); d.emp = r.put(p.edge_mp, nE);
+    d.pt_off = r.put(ptOff.data(), (size_t)nMP + 1); d.pt_edge = r.put(ptEdge.data(), nE);
+    d.kf_off = r.put(kfOff.data(), (size_t)nKF + 1); d.kf_edge = r.put(kfEdge.data(), nE);
+    d.kl_off = r.put(klOff.data(), (size_t)nKF + 1); d.kl_ent = r.put(klEnt.data(), 2 * (size_t)nL);
+    d.pair_p = r.put(pairP.data(), nPairs); d.pair_off = r.put(pairOff.data(), (size_t)nPairs + 1);
+    d.co_e1 = r.put(coE1.data(), nCo); d.co_e2 = r.put(coE2.data(), nCo);
+    lay.in_bytes = r.bytes() - lay.io_bytes;
+    d.state_saved = r.take<double>(21 * (size_t)nKF); d.point_saved = r.take<double>(sl);
+    d.Hpp = r.take<double>(sp * sp); d.Hs = r.take<double>(sp * sp);
+    d.b = r.take<double>(sp + sl); d.bs = r.take<double>(sp);
+    d.x = r.take<double>(sp + sl); d.y = r.take<double>(sp);
+    d.Hll = r.take<double>(9 * (size_t)nMP); d.Dinv = r.take<double>(9 * (size_t)nMP);
+    d.W = r.take<double>(18 * (size_t)nE); d.WD = r.take<double>(18 * (size_t)nE);
+    d.Wdb = r.take<double>(6 * (size_t)nE); d.Epp = r.take<double>(27 * (size_t)nE);
+    d.Lblk = r.take<double>(930 * (size_t)nL);
+    d.flag = r.take<int>(4); d.partials = r.take<double>(16); d.part = r.take<double>((size_t)LIBA_CHUNKS * std::max((size_t)27 * nKF, (size_t)36 * nPairs));
+    d.part_b = r.take<double>((size_t)LIBA_CHUNKS * 6 * nKF); d.Ypan = r.take<double>(15 * sp);
+    lay.total = r.bytes();
+    lay.work_bytes = lay.total - lay.io_bytes - lay.in_bytes;
+    if (!dev) return lay;
 
-    memset(host, 0, lay.io_bytes + lay.in_bytes);
-    auto put = [&](size_t o, const void* src, size_t bytes) { if (bytes) memcpy(host + o, src, bytes); };
-    put(oState, p.state, 8 * 21 * (size_t)nKF);
-    put(oPoint, p.point, 8 * sl);
-    put(oObs, p.obs, 8 * 3 * (size_t)nE);
-    put(oInv, p.inv_sigma2, 8 * (size_t)nE);
-    put(oLinks, p.links, sizeof(LibaLink) * (size_t)nL);
-    put(oPidx, pidx.data(), 4 * (size_t)nKF);
-    put(oEkf, p.edge_kf, 4 * (size_t)nE);
-    put(oEmp, p.edge_mp, 4 * (size_t)nE);
-    put(oPtOff, ptOff.data(), 4 * ((size_t)nMP + 1));
-    put(oPtEdge, ptEdge.data(), 4 * (size_t)nE);
-    put(oKfOff, kfOff.data(), 4 * ((size_t)nKF + 1));
-    put(oKfEdge, kfEdge.data(), 4 * (size_t)nE);
-    put(oKlOff, klOff.data(), 4 * ((size_t)nKF + 1));
-    put(oKlEnt, klEnt.data(), 4 * 2 * (size_t)nL);
-    put(oPairP, pairP.data(), 4 * (size_t)nPairs);
-    put(oPairOff, pairOff.data(), 4 * ((size_t)nPairs + 1));
-    put(oCo1, coE1.data(), 4 * nCo);
-    put(oCo2, coE2.data(), 4 * nCo);
-
-    LibaDev& d = *dev;
     d.nKF = nKF; d.nMP = nMP; d.nE = nE; d.nL = nL; d.nFree = nFree; d.sp = (int)sp; d.nPairs = nPairs;
-    auto D = [&](size_t o) { return reinterpret_cast<double*>(devBase + o); };
-    auto I = [&](size_t o) { return reinterpret_cast<int*>(devBase + o); };
-    d.state = D(oState); d.state_saved = D(oStateS); d.point = D(oPoint); d.point_saved = D(oPointS);
-    d.pidx = I(oPidx); d.ekf = I(oEkf); d.emp = I(oEmp); d.obs = D(oObs); d.invs2 = D(oInv); d.pt_off = I(oPtOff); d.pt_edge = I(oPtEdge);
-    d.kf_off = I(oKfOff); d.kf_edge = I(oKfEdge); d.kl_off = I(oKlOff); d.kl_ent = I(oKlEnt);
-    d.pair_p = I(oPairP); d.pair_off = I(oPairOff); d.co_e1 = I(oCo1); d.co_e2 = I(oCo2);
-    d.links = reinterpret_cast<const LibaLink*>(devBase + oLinks);
     for (int i = 0; i < 9; ++i) d.Rcb[i] = p.Tcb[i];
     for (int i = 0; i < 3; ++i) d.tcb[i] = p.Tcb[9 + i];
     m3_T(d.Rcb, d.Rbc);
@@ -135,10 +115,9 @@ inline LibaLayout liba_pack(const liba_problem& p, uint8_t* host, uint8_t* devBa
     d.fx = p.fx; d.fy = p.fy; d.cx = p.cx; d.cy = p.cy; d.bf = p.bf;
     d.lambda_init = p.lambda_init;
     d.max_iters = p.max_iters;
-    d.err = D(oErr); d.lerr = D(oLerr); d.Hpp = D(oHpp); d.Hs = D(oHs); d.b = D(oB); d.bs = D(oBs); d.x = D(oX); d.y = D(oY);
-    d.Hll = D(oHll); d.Dinv = D(oDinv); d.W = D(oW); d.WD = D(oWD); d.Wdb = D(oWdb); d.Epp = D(oEpp); d.Lblk = D(oLblk); d.part = D(oChunk); d.part_b = D(oChunkB); d.Ypan = D(oYpan);
-    d.flag = I(oFlag); d.red = nullptr; d.partials = D(oPart); d.out_scalars = D(oOut); d.dpos = devBase + oDpos;
+    d.red = nullptr;
     d.t_id = 0; d.t_stride = 1; d.l_id = 0; d.l_stride = 1; d.rank = 0; d.cs = 1;      // a team of one thread; the launcher overrides per thread
+    *dev = d;
     return lay;
 }
 

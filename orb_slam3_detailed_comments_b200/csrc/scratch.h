@@ -11,10 +11,12 @@
 // | `h->d_stage` | every matcher.cu entry point, `orbm_search_triangulation`, `orbo_pose_optimization`, `orbo_pose_edges` (its count array) |
 // | `h->d_po` | `orbo_pose_optimization_frames` (it calls the two above), `orbv_transform`, `orbp_distinctive_descriptors`, `orbp_update_normal_and_depth`, `orbm_hamming_knn2` |
 // | `orbr_state::d_buf` | `orbr_submit` (it calls the searches and pose calls above) |
-// | `lba_handle` / `liba_handle` `d_buf`, `h_buf` | `lba_solve*`, `liba_solve` |
 // | `h->d_xl` | the frame blocks of the matcher searches' global-memory form (matcher.cu `launch_proj`) |
 //
 // Captured CUDA graphs hold pointers into these buffers, so a buffer only grows in an eager call: growth inside a capture is refused.
+//
+// The two bundle-adjustment solvers (`lba_solve*`, `liba_solve`) are not carved: each lays a batch out in its handle's `d_buf` with
+// a pinned mirror in `h_buf` (pack.h), both grown by the functions below.
 #pragma once
 #include <algorithm>
 
@@ -77,6 +79,49 @@ inline orb_status grow_pinned(size_t& bytes, uint8_t*& ptr, size_t need) {
     ORB_CUDA(cudaMallocHost((void**)&ptr, want));
     bytes = want;
     return ORB_OK;
+}
+
+// What a solver handle (lba_handle, liba_handle) holds besides its own state.
+struct SolverHandle {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    uint8_t* d_buf = nullptr;   // device block of a batch
+    size_t d_bytes = 0;
+    uint8_t* h_buf = nullptr;   // its pinned mirror
+    size_t h_bytes = 0;
+    int n_sms = 1;
+};
+
+// Creates *out on `device` with its own stream; `kern` may then be launched in clusters of up to 16 CTAs and with up to
+// `max_smem` bytes of dynamic shared memory (0: the default limit).
+template <typename H, typename... KArgs>
+orb_status solver_create(int32_t device, void (*kern)(KArgs...), size_t max_smem, H** out) {
+    if (!out) return set_error(ORB_ERR_INVALID, "null argument");
+    *out = nullptr;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
+        return set_error(ORB_ERR_NO_DEVICE, "no usable CUDA device (this library has no CPU fallback)");
+    ORB_CUDA(cudaSetDevice(device));
+    ORB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    if (max_smem) ORB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem));
+    H* h = new H();
+    h->device = device;
+    h->n_sms = device_sm_count(device);
+    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
+        delete h;
+        return set_error(ORB_ERR_CUDA, "cudaStreamCreate failed");
+    }
+    *out = h;
+    return ORB_OK;
+}
+
+// Waits for the handle's work and frees what solver_create and the solves allocated; the caller frees its own state, then deletes.
+inline void solver_release(SolverHandle* h) {
+    cudaSetDevice(h->device);
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    if (h->d_buf) cudaFree(h->d_buf);
+    if (h->h_buf) cudaFreeHost(h->h_buf);
+    if (h->stream) cudaStreamDestroy(h->stream);
 }
 
 // measure `layout`, grow the buffer to fit, carve it: returns the first error of the growth or of a stage_in copy

@@ -244,6 +244,43 @@ extern "C" void emul_liba_inertial(const double* state2x21, const liba_link* lin
 
 extern "C" size_t emul_liba_layout_total(const liba_problem* p) { return orb::liba_pack(*p, nullptr, nullptr, nullptr).total; }
 
+// ---- LocalBundleAdjustment: the index structures and the batch layout of csrc/lba_pack.h ----------------------------------------
+#include "../../orb_slam3_detailed_comments_b200/csrc/lba_pack.h"
+
+#define EMUL_LBA_POINTERS(X) X(pose0) X(point0) X(pidx) X(ekf) X(emp) X(obs) X(invs2) X(mpStart) X(mpEdge) X(poseStart) X(poseEdge) \
+    X(pairStart) X(ptItemStart) X(ptItem) X(taskStart) X(blockTask) X(taskSum) X(BD) X(poseSlot) X(blockP1) X(blockP2) X(pose)      \
+    X(point) X(poseSave) X(pointSave) X(Hpl) X(W) X(Prod) X(Hll) X(bl) X(Dinv) X(db) X(Hpp) X(bp) X(xl) X(HsGlobal) X(posePart)       \
+    X(HsBlocks) X(bs) X(xp) X(partials) X(flags) X(err) X(depthPos) X(stats)
+#define EMUL_LBA_INTS(X) X(nKF) X(nMP) X(nE) X(nP) X(n) X(nItems) X(nTasks) X(nFreeEdges) X(nPairBlocks)
+#define EMUL_LBA_NAME(m) #m " "
+
+// the descriptor members emul_lba_pack exports, in its order
+extern "C" const char* emul_lba_fields() { return EMUL_LBA_POINTERS(EMUL_LBA_NAME) EMUL_LBA_INTS(EMUL_LBA_NAME); }
+
+// lba_prepare + lba_pack of n problems with blob as both the host mirror and the device block: blob == nullptr measures.
+// sizes = in, desc, work bytes; fields[n][emul_lba_fields]: the blob offset a pointer member points at (-1: null), then the ints.
+// Returns lba_prepare's status of the first problem it refuses.
+extern "C" int emul_lba_pack(const lba_problem* p, int n, uint8_t* blob, int64_t* sizes, int64_t* fields) {
+    std::vector<orb::LbaPrep> prep(n);
+    for (int i = 0; i < n; ++i) {
+        const char* why = nullptr;
+        const orb_status s = orb::lba_prepare(p[i], prep[i], &why);
+        if (s != ORB_OK) return s;
+    }
+    const orb::LbaLayout lay = orb::lba_pack(n, p, prep.data(), nullptr, blob, blob);
+    sizes[0] = (int64_t)lay.in_bytes; sizes[1] = (int64_t)lay.desc_bytes; sizes[2] = (int64_t)lay.work_bytes;
+    if (!blob) return ORB_OK;
+    const orb::LbaDev* D = reinterpret_cast<const orb::LbaDev*>(blob + lay.in_bytes);
+    int64_t* f = fields;
+    for (int i = 0; i < n; ++i) {
+#define EMUL_LBA_PTR(m) *f++ = D[i].m ? (int64_t)((const uint8_t*)D[i].m - blob) : -1;
+#define EMUL_LBA_INT(m) *f++ = D[i].m;
+        EMUL_LBA_POINTERS(EMUL_LBA_PTR)
+        EMUL_LBA_INTS(EMUL_LBA_INT)
+    }
+    return ORB_OK;
+}
+
 // ---- Frame::ComputeStereoMatches, variant 1: csrc/stereo_core.cuh (the body of k_stereo_match_v1's threads) on the host ----------------
 #include "../../orb_slam3_detailed_comments_b200/csrc/stereo_core.cuh"
 
