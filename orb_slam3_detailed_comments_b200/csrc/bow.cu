@@ -188,16 +188,17 @@ extern "C" orb_status orbv_transform(orbx_handle* h, const orbv_vocabulary* voc,
     P.offsets = h->d_offsets; P.nkp = h->d_nkp; P.maxFeat = maxFeat;
     // results staging shares the pose-optimisation buffer (not the matcher stage: its feature_node input may live there)
     auto layout = [&](Carve& c) {
-        P.word = dev ? word_out : c.take<int>(rows);
-        P.node = dev ? node_out : c.take<int>(rows);
-        P.weight = dev ? weight_out : c.take<double>(rows);
+        P.word = stage_out(c, word_out, rows, dev);
+        P.node = stage_out(c, node_out, rows, dev);
+        P.weight = stage_out(c, weight_out, rows, dev);
         if (want_bow) {
-            P.bow_count = dev ? bow_count_out : c.take<int>(nimg);
-            P.bow_word = dev ? bow_word_out : c.take<int>((size_t)nimg * maxFeat);
-            P.bow_weight = dev ? bow_weight_out : c.take<double>((size_t)nimg * maxFeat);
+            P.bow_count = stage_out(c, bow_count_out, nimg, dev);
+            P.bow_word = stage_out(c, bow_word_out, (size_t)nimg * maxFeat, dev);
+            P.bow_weight = stage_out(c, bow_weight_out, (size_t)nimg * maxFeat, dev);
         }
     };
-    if ((s = carve_scratch(h->po_bytes, h->d_po, h->capturing, h->stream, layout)) != ORB_OK) return s;
+    const Carve c = carve_scratch(h->po_bytes, h->d_po, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
     cudaStream_t st = h->stream;
     if (rows > 0) {
         k_bow_transform<<<(rows * 16 + 255) / 256, 256, 0, st>>>(P);
@@ -209,18 +210,5 @@ extern "C" orb_status orbv_transform(orbx_handle* h, const orbv_vocabulary* voc,
         ORB_LAUNCHED();
     }
     ORB_CUDA(cudaGetLastError());
-    if (!dev) {
-        if (rows > 0) {
-            ORB_CUDA(cudaMemcpyAsync(word_out, P.word, sizeof(int) * (size_t)rows, cudaMemcpyDeviceToHost, st));
-            ORB_CUDA(cudaMemcpyAsync(node_out, P.node, sizeof(int) * (size_t)rows, cudaMemcpyDeviceToHost, st));
-            ORB_CUDA(cudaMemcpyAsync(weight_out, P.weight, sizeof(double) * (size_t)rows, cudaMemcpyDeviceToHost, st));
-        }
-        if (want_bow) {
-            ORB_CUDA(cudaMemcpyAsync(bow_count_out, P.bow_count, sizeof(int) * (size_t)nimg, cudaMemcpyDeviceToHost, st));
-            ORB_CUDA(cudaMemcpyAsync(bow_word_out, P.bow_word, sizeof(int) * (size_t)nimg * maxFeat, cudaMemcpyDeviceToHost, st));
-            ORB_CUDA(cudaMemcpyAsync(bow_weight_out, P.bow_weight, sizeof(double) * (size_t)nimg * maxFeat, cudaMemcpyDeviceToHost, st));
-        }
-        ORB_CUDA(cudaStreamSynchronize(st));
-    }
-    return ORB_OK;
+    return dev ? ORB_OK : copy_out(c);
 }

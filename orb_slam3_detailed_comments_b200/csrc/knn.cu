@@ -184,18 +184,15 @@ extern "C" orb_status orbm_hamming_knn2(orbx_handle* h, int32_t n_pairs, const i
         P.q_off = stage_in(c, query_offset, np + 1, false); P.t_off = stage_in(c, train_offset, np + 1, false);
         P.q_desc = stage_in(c, query_desc, (size_t)nq * 32, false);
         P.t_desc = train_desc ? stage_in(c, train_desc, (size_t)nt * 32, false) : c.take<uint8_t>(32);   // a real address even with no train rows
-        P.idx = c.take<int>((size_t)nq * 2);
-        P.dist = c.take<int>((size_t)nq * 2);
+        P.idx = stage_out(c, idx_out, (size_t)nq * 2, false);
+        P.dist = stage_out(c, dist_out, (size_t)nq * 2, false);
     };
-    const orb_status s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
-    if (s != ORB_OK) return s;
+    const Carve c = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
+    if (c.status != ORB_OK) return c.status;
     const char* tma = getenv("ORB_KNN_TMA");       // 1: train tiles by cp.async.bulk + mbarrier, double-buffered
     if (tma && atoi(tma) == 1) k_hamming_knn2_tma<<<dim3((maxq + KNN_THREADS - 1) / KNN_THREADS, n_pairs), KNN_THREADS, 0, st>>>(P);
     else k_hamming_knn2<<<dim3((maxq + KNN_THREADS - 1) / KNN_THREADS, n_pairs), KNN_THREADS, 0, st>>>(P);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
-    ORB_CUDA(cudaMemcpyAsync(idx_out, P.idx, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaMemcpyAsync(dist_out, P.dist, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaStreamSynchronize(st));
-    return ORB_OK;
+    return copy_out(c);
 }

@@ -90,17 +90,15 @@ extern "C" orb_status orbp_distinctive_descriptors(orbx_handle* h, int32_t n_poi
     const int* d_off; const uint8_t* d_desc; int* d_best;
     auto layout = [&](Carve& c) {
         d_off = stage_in(c, obs_offset, (size_t)n_points + 1, false);
-        d_best = c.take<int>(n_points);
+        d_best = stage_out(c, best_index_out, n_points, false);
         d_desc = stage_in(c, obs_desc, (size_t)nobs * 32, false);
     };
-    const orb_status s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
-    if (s != ORB_OK) return s;
+    const Carve c = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
+    if (c.status != ORB_OK) return c.status;
     k_distinctive<<<n_points, 32, 0, st>>>(d_off, d_desc, d_best);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
-    ORB_CUDA(cudaMemcpyAsync(best_index_out, d_best, sizeof(int) * (size_t)n_points, cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaStreamSynchronize(st));
-    return ORB_OK;
+    return copy_out(c);
 }
 
 extern "C" orb_status orbp_update_normal_and_depth(orbx_handle* h, int32_t n_points, const int32_t* obs_offset, const float* obs_center,
@@ -123,15 +121,12 @@ extern "C" orb_status orbp_update_normal_and_depth(orbx_handle* h, int32_t n_poi
         d_lv = stage_in(c, ref_level, np, false); d_sc = stage_in(c, h->scale.data(), (size_t)h->cfg.n_levels, false);
         // outputs start from the caller's current values: points without observations keep them
         d_n = stage_in(c, normal_out, np * 3, false); d_mx = stage_in(c, max_dist_out, np, false); d_mn = stage_in(c, min_dist_out, np, false);
+        c.copy_back(normal_out, d_n, np * 3); c.copy_back(max_dist_out, d_mx, np); c.copy_back(min_dist_out, d_mn, np);
     };
-    const orb_status s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
-    if (s != ORB_OK) return s;
+    const Carve c = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
+    if (c.status != ORB_OK) return c.status;
     k_normal_depth<<<(n_points + 127) / 128, 128, 0, st>>>(n_points, d_off, d_oc, d_pos, d_rc, d_lv, d_sc, h->cfg.n_levels, d_n, d_mx, d_mn);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
-    ORB_CUDA(cudaMemcpyAsync(normal_out, d_n, np * 12, cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaMemcpyAsync(max_dist_out, d_mx, np * 4, cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaMemcpyAsync(min_dist_out, d_mn, np * 4, cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaStreamSynchronize(st));
-    return ORB_OK;
+    return copy_out(c);
 }

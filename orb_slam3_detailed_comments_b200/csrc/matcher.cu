@@ -217,25 +217,31 @@ __global__ void __launch_bounds__(256) k_in_frustum(const __grid_constant__ Frus
 // ------------------------------------------------------------------------------------------------
 // Runs one search.  The call's shared-memory need (the largest block its kernels ask for) decides the form, once per call: the
 // shared-memory form whenever the device can give it, else the global-memory form (*_xl), whose frame blocks live in
-// h->d_xl and whose kernels keep only the per-feature resolve state in shared memory.  Both compute the same matches.
-static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int max_q_per_frame) {
+// h->d_xl and whose kernels keep only the per-feature resolve state in shared memory.  Both compute the same matches.  A search
+// without queries launches nothing and zeroes its counts, so no caller sees an earlier call's.
+static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int n_queries, int max_q_per_frame) {
     cudaStream_t st = h->stream;
-    const size_t fsm = ((size_t)P.maxFeat * 23 + 16 + 15) / 16 * 16;
-    const size_t gsm = ((size_t)P.maxFeat * 17 + (PM_NCELL + 1) * 2 + 32 + 15) / 16 * 16;
+    if (n_queries == 0) {
+        ORB_CUDA(cudaMemsetAsync(P.nmatches, 0, sizeof(int) * n_frames, st));
+        return ORB_OK;
+    }
+    const size_t fsm = ((size_t)P.maxFeat * 23 + 16 + 15) / 16 * 16;                       // the staged frame
+    const size_t gsm = ((size_t)P.maxFeat * 17 + (PM_NCELL + 1) * 2 + 32 + 15) / 16 * 16;  // the staged grid
     const size_t csm = std::max(fsm, gsm);
-    const size_t psm = fsm + (size_t)P.maxFeat * 9 + (size_t)(PR_QCAP + PR_LIST) * 4 + 64;
-    const size_t rsm = fsm + (size_t)PM_CHUNK * PM_K * 8 + (size_t)PM_CHUNK * 4 + (size_t)P.maxFeat * (P.mode == 4 ? 9 : 5) + (size_t)PM_CHUNK * 5 + 256;
+    // the resolve kernels' own arrays, after the staged frame
+    const size_t pown = (size_t)P.maxFeat * 9 + (size_t)(PR_QCAP + PR_LIST) * 4 + 64;
+    const size_t rown = (size_t)PM_CHUNK * PM_K * 8 + (size_t)PM_CHUNK * 4 + (size_t)P.maxFeat * (P.mode == 4 ? 9 : 5) + (size_t)PM_CHUNK * 5 + 256;
     // static __shared__ arrays count against the same limit; the *_xl kernels share the resolve bodies and so their static arrays
     static const size_t candStatic = std::max({static_smem(k_proj_candidates), static_smem(k_proj_candidates_grp<4>),
                                                static_smem(k_proj_candidates_grp<8>), static_smem(k_proj_candidates_grp<16>)});
     static const size_t parStatic = static_smem(k_proj_resolve_par), resStatic = static_smem(k_proj_resolve);
     const size_t optin = (size_t)smem_optin(h);
-    const bool global = csm + candStatic > optin || (P.seqFlag && psm + parStatic > optin) || rsm + resStatic > optin;
+    const bool global = csm + candStatic > optin || (P.seqFlag && fsm + pown + parStatic > optin) || fsm + rown + resStatic > optin;
     GlobalFrame S{};
     orb_status s;
-    if (global) {   // the same kernels without the staged frame (fsm) in shared memory
-        if ((P.seqFlag && (s = check_smem(h, psm - fsm, parStatic, "k_proj_resolve_par_xl")) != ORB_OK) ||
-            (s = check_smem(h, rsm - fsm, resStatic, "k_proj_resolve_xl")) != ORB_OK)
+    if (global) {   // the same kernels without the staged frame in shared memory
+        if ((P.seqFlag && (s = check_smem(h, pown, parStatic, "k_proj_resolve_par_xl")) != ORB_OK) ||
+            (s = check_smem(h, rown, resStatic, "k_proj_resolve_xl")) != ORB_OK)
             return s;
         S.featStride = (fsm + 255) / 256 * 256;
         S.gridStride = (gsm + 255) / 256 * 256;
@@ -243,8 +249,20 @@ static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int m
             S.featBlocks = c.take<unsigned char>((size_t)n_frames * S.featStride);
             S.gridBlocks = P.mode != 2 ? c.take<unsigned char>((size_t)n_frames * S.gridStride) : nullptr;
         };
-        if ((s = carve_scratch(h->xl_bytes, h->d_xl, h->capturing, st, layout)) != ORB_OK) return s;
+        if ((s = carve_scratch(h->xl_bytes, h->d_xl, h->capturing, st, layout).status) != ORB_OK) return s;
     }
+    // One kernel role: the shared-memory kernel with `staged` bytes of frame or grid ahead of its `own` bytes, or its *_xl twin with
+    // only its own bytes and the frame blocks S.  An empty grid launches nothing.
+    auto run = [&](auto kern, auto kern_xl, dim3 grid, int threads, size_t staged, size_t own) -> orb_status {
+        const size_t smem = global ? own : staged + own;
+        if (smem) ORB_CUDA(global ? cudaFuncSetAttribute(kern_xl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                                  : cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if (grid.x == 0) return ORB_OK;
+        if (global) launch_p(kern_xl, grid, dim3(threads), smem, st, P, S);
+        else launch_p(kern, grid, dim3(threads), smem, st, P);
+        ORB_LAUNCHED();
+        return ORB_OK;
+    };
     if (P.mode != 2) {   // modes 0, 1, 3 search a window of the feature grid
         const size_t gridSm = (size_t)(PM_NCELL + 2) * 4 + (size_t)P.maxFeat * 4 + 16;
         static const size_t gridStatic = static_smem(k_frame_grid);
@@ -262,58 +280,18 @@ static orb_status launch_proj(orbx_handle* h, ProjParams& P, int n_frames, int m
     const char* vQpb = getenv("ORB_PROJ_QPB");
     const int envLanes = vLanes ? atoi(vLanes) : 0, envQpb = vQpb ? atoi(vQpb) : 0;
     const int lanes = P.mode > 1 ? 32 : (envLanes ? envLanes : (P.mode == 0 ? 4 : 8));
+    auto cand = k_proj_candidates;
+    auto cand_xl = k_proj_candidates_xl;
+    int qpb = PM_QPB;
     if (lanes == 4 || lanes == 8 || lanes == 16) {
-        P.qpb = envQpb > 0 ? envQpb : (P.mode == 0 ? 128 : 64);
-        dim3 grid((max_q_per_frame + P.qpb - 1) / P.qpb, n_frames);
-        if (global) {
-            auto kern = lanes == 4 ? k_proj_candidates_grp_xl<4> : (lanes == 8 ? k_proj_candidates_grp_xl<8> : k_proj_candidates_grp_xl<16>);
-            if (grid.x > 0) {
-                launch_p(kern, grid, dim3(PM_WARPS * 32), 0, st, P, S);
-                ORB_LAUNCHED();
-            }
-        } else {
-            auto kern = lanes == 4 ? k_proj_candidates_grp<4> : (lanes == 8 ? k_proj_candidates_grp<8> : k_proj_candidates_grp<16>);
-            ORB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(csm, (size_t)1024)));
-            if (grid.x > 0) {
-                launch_p(kern, grid, dim3(PM_WARPS * 32), csm, st, P);
-                ORB_LAUNCHED();
-            }
-        }
-    } else {
-        dim3 grid((max_q_per_frame + PM_QPB - 1) / PM_QPB, n_frames);
-        if (global) {
-            if (grid.x > 0) {
-                launch_p(k_proj_candidates_xl, grid, dim3(PM_WARPS * 32), 0, st, P, S);
-                ORB_LAUNCHED();
-            }
-        } else {
-            ORB_CUDA(cudaFuncSetAttribute(k_proj_candidates, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(csm, (size_t)1024)));
-            if (grid.x > 0) {
-                k_proj_candidates<<<grid, PM_WARPS * 32, csm, st>>>(P);
-                ORB_LAUNCHED();
-            }
-        }
+        qpb = P.qpb = envQpb > 0 ? envQpb : (P.mode == 0 ? 128 : 64);
+        cand = lanes == 4 ? k_proj_candidates_grp<4> : (lanes == 8 ? k_proj_candidates_grp<8> : k_proj_candidates_grp<16>);
+        cand_xl = lanes == 4 ? k_proj_candidates_grp_xl<4> : (lanes == 8 ? k_proj_candidates_grp_xl<8> : k_proj_candidates_grp_xl<16>);
     }
-    if (global) {
-        ORB_CUDA(cudaFuncSetAttribute(k_proj_resolve_par_xl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(psm - fsm)));
-        ORB_CUDA(cudaFuncSetAttribute(k_proj_resolve_xl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(rsm - fsm)));
-        if (P.seqFlag) {
-            launch_p(k_proj_resolve_par_xl, dim3(n_frames), dim3(PR_THREADS), psm - fsm, st, P, S);
-            ORB_LAUNCHED();
-        }
-        launch_p(k_proj_resolve_xl, dim3(n_frames), dim3(256), rsm - fsm, st, P, S);
-        ORB_LAUNCHED();
-        ORB_CUDA(cudaGetLastError());
-        return ORB_OK;
-    }
-    if (P.seqFlag) {   // modes 0 / 1: parallel fixed-point resolve; frames it cannot finish are flagged for the sequential kernel
-        ORB_CUDA(cudaFuncSetAttribute(k_proj_resolve_par, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-        launch_p(k_proj_resolve_par, dim3(n_frames), dim3(PR_THREADS), psm, st, P);
-        ORB_LAUNCHED();
-    }
-    ORB_CUDA(cudaFuncSetAttribute(k_proj_resolve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsm));
-    launch_p(k_proj_resolve, dim3(n_frames), dim3(256), rsm, st, P);
-    ORB_LAUNCHED();
+    if ((s = run(cand, cand_xl, dim3((max_q_per_frame + qpb - 1) / qpb, n_frames), PM_WARPS * 32, csm, 0)) != ORB_OK) return s;
+    // modes 0 / 1: parallel fixed-point resolve; frames it cannot finish are flagged for the sequential kernel
+    if (P.seqFlag && (s = run(k_proj_resolve_par, k_proj_resolve_par_xl, dim3(n_frames), PR_THREADS, fsm, pown)) != ORB_OK) return s;
+    if ((s = run(k_proj_resolve, k_proj_resolve_xl, dim3(n_frames), 256, fsm, rown)) != ORB_OK) return s;
     ORB_CUDA(cudaGetLastError());
     return ORB_OK;
 }
@@ -392,21 +370,15 @@ extern "C" orb_status orbm_search_local_points(orbx_handle* h, const orbm_camera
         P.gridStart = c.take<uint16_t>((size_t)nf * (GRID_COLS * GRID_ROWS + 1));
         P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
         P.cnt = c.take<int>(nq);
-        P.match = dev ? match_out : c.take<int>(nq);
-        P.nmatches = (dev && nmatches_out) ? nmatches_out : c.take<int>(nf);
+        P.match = stage_out(c, match_out, nq, dev);
+        P.nmatches = stage_out(c, nmatches_out, nf, dev);
         P.seqFlag = c.take<int>(nf);
     };
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
     ORB_CUDA(cudaMemsetAsync(P.seqFlag, 0, sizeof(int) * nf, h->stream));
-    if (nq > 0 && (s = launch_proj(h, P, nf, maxq)) != ORB_OK) return s;
-    if (dev && nq == 0 && nmatches_out) ORB_CUDA(cudaMemsetAsync(nmatches_out, 0, sizeof(int) * nf, h->stream));   // no kernel ran: a consumer must not see the previous step's counts
-    if (!dev) {
-        if (nq > 0) ORB_CUDA(cudaMemcpyAsync(match_out, P.match, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, h->stream));
-        if (nmatches_out && nq > 0) ORB_CUDA(cudaMemcpyAsync(nmatches_out, P.nmatches, sizeof(int) * nf, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-        if (nmatches_out && nq == 0) std::fill(nmatches_out, nmatches_out + nf, 0);
-    }
-    return ORB_OK;
+    if ((s = launch_proj(h, P, nf, nq, maxq)) != ORB_OK) return s;
+    return dev ? ORB_OK : copy_out(c);
 }
 
 extern "C" orb_status orbm_search_last_frame(orbx_handle* h, const orbm_camera* cam, const orbm_last_queries* Q, float th,
@@ -437,20 +409,16 @@ extern "C" orb_status orbm_search_last_frame(orbx_handle* h, const orbm_camera* 
         P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
         P.cnt = c.take<int>(nq);
         P.quv = c.take<float>(nq);
-        P.match = dev ? feature_match_out : c.take<int>(total_rows);
-        P.nmatches = (dev && nmatches_out) ? nmatches_out : c.take<int>(nf);
+        P.match = stage_out(c, feature_match_out, total_rows, dev);
+        P.nmatches = stage_out(c, nmatches_out, nf, dev);
         P.seqFlag = c.take<int>(nf);
     };
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
     ORB_CUDA(cudaMemsetAsync(P.match, 0xff, sizeof(int) * (size_t)total_rows, h->stream));
     ORB_CUDA(cudaMemsetAsync(P.seqFlag, 0, sizeof(int) * nf, h->stream));
-    if ((s = launch_proj(h, P, nf, maxq)) != ORB_OK) return s;
-    if (!dev) {
-        ORB_CUDA(cudaMemcpyAsync(feature_match_out, P.match, sizeof(int) * (size_t)total_rows, cudaMemcpyDeviceToHost, h->stream));
-        if (nmatches_out) ORB_CUDA(cudaMemcpyAsync(nmatches_out, P.nmatches, sizeof(int) * nf, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-    }
-    return ORB_OK;
+    if ((s = launch_proj(h, P, nf, nq, maxq)) != ORB_OK) return s;
+    return dev ? ORB_OK : copy_out(c);
 }
 
 extern "C" orb_status orbm_search_bow(orbx_handle* h, const orbm_bow_queries* Q, float nnratio, int32_t check_orientation,
@@ -477,18 +445,14 @@ extern "C" orb_status orbm_search_bow(orbx_handle* h, const orbm_bow_queries* Q,
         P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
         P.cnt = c.take<int>(nq);
         P.quv = c.take<float>(nq);
-        P.match = dev ? feature_match_out : c.take<int>(total_rows);
-        P.nmatches = (dev && nmatches_out) ? nmatches_out : c.take<int>(nf);
+        P.match = stage_out(c, feature_match_out, total_rows, dev);
+        P.nmatches = stage_out(c, nmatches_out, nf, dev);
     };
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
     ORB_CUDA(cudaMemsetAsync(P.match, 0xff, sizeof(int) * (size_t)total_rows, h->stream));
-    if ((s = launch_proj(h, P, nf, maxq)) != ORB_OK) return s;
-    if (!dev) {
-        ORB_CUDA(cudaMemcpyAsync(feature_match_out, P.match, sizeof(int) * (size_t)total_rows, cudaMemcpyDeviceToHost, h->stream));
-        if (nmatches_out) ORB_CUDA(cudaMemcpyAsync(nmatches_out, P.nmatches, sizeof(int) * nf, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-    }
-    return ORB_OK;
+    if ((s = launch_proj(h, P, nf, nq, maxq)) != ORB_OK) return s;
+    return dev ? ORB_OK : copy_out(c);
 }
 
 extern "C" orb_status orbm_search_keyframe(orbx_handle* h, const orbm_camera* cam, const orbm_kf_queries* Q, int32_t variant,
@@ -558,18 +522,13 @@ extern "C" orb_status orbm_search_keyframe(orbx_handle* h, const orbm_camera* ca
         P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
         P.cnt = c.take<int>(nq);
         P.quv = c.take<float>(nq);
-        P.match = c.take<int>(nq);
-        P.nmatches = c.take<int>(nt);
+        P.match = stage_out(c, match_out, nq, false);
+        P.nmatches = stage_out(c, nmatches_out, nt, false);
     };
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
-    if (nq > 0) {
-        if ((s = launch_proj(h, P, nt, maxq)) != ORB_OK) return s;
-        ORB_CUDA(cudaMemcpyAsync(match_out, P.match, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, h->stream));
-        if (nmatches_out) ORB_CUDA(cudaMemcpyAsync(nmatches_out, P.nmatches, sizeof(int) * nt, cudaMemcpyDeviceToHost, h->stream));
-    }
-    ORB_CUDA(cudaStreamSynchronize(h->stream));   // also keeps the host vectors alive until the uploads are done
-    if (nmatches_out && nq == 0) std::fill(nmatches_out, nmatches_out + nt, 0);
-    return ORB_OK;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
+    if ((s = launch_proj(h, P, nt, nq, maxq)) != ORB_OK) return s;
+    return copy_out(c);   // also keeps the host vectors alive until the uploads are done
 }
 
 extern "C" orb_status orbm_search_bow_keyframes(orbx_handle* h, const orbm_bow_kf_queries* Q, float nnratio, int32_t check_orientation,
@@ -614,18 +573,13 @@ extern "C" orb_status orbm_search_bow_keyframes(orbx_handle* h, const orbm_bow_k
         P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
         P.cnt = c.take<int>(nq);
         P.quv = c.take<float>(nq);
-        P.match = c.take<int>(nq);
-        P.nmatches = c.take<int>(nt);
+        P.match = stage_out(c, match12_out, nq, false);
+        P.nmatches = stage_out(c, nmatches_out, nt, false);
     };
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
-    if (nq > 0) {
-        if ((s = launch_proj(h, P, nt, maxq)) != ORB_OK) return s;
-        ORB_CUDA(cudaMemcpyAsync(match12_out, P.match, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, h->stream));
-        if (nmatches_out) ORB_CUDA(cudaMemcpyAsync(nmatches_out, P.nmatches, sizeof(int) * nt, cudaMemcpyDeviceToHost, h->stream));
-    }
-    ORB_CUDA(cudaStreamSynchronize(h->stream));
-    if (nmatches_out && nq == 0) std::fill(nmatches_out, nmatches_out + nt, 0);
-    return ORB_OK;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
+    if ((s = launch_proj(h, P, nt, nq, maxq)) != ORB_OK) return s;
+    return copy_out(c);
 }
 
 extern "C" orb_status orbm_search_initialization(orbx_handle* h, const orbm_camera* cam, const orbm_init_queries* Q, int32_t window_size,
@@ -677,18 +631,13 @@ extern "C" orb_status orbm_search_initialization(orbx_handle* h, const orbm_came
         P.topk = c.take<unsigned long long>((size_t)nq * PM_K);
         P.cnt = c.take<int>(nq);
         P.quv = c.take<float>(nq);
-        P.match = c.take<int>(nq);
-        P.nmatches = c.take<int>(1);
+        P.match = stage_out(c, matches12_out, nq, false);
+        P.nmatches = stage_out(c, nmatches_out, 1, false);
     };
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
-    if (nq > 0) {
-        if ((s = launch_proj(h, P, 1, nq)) != ORB_OK) return s;
-        ORB_CUDA(cudaMemcpyAsync(matches12_out, P.match, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, h->stream));
-        if (nmatches_out) ORB_CUDA(cudaMemcpyAsync(nmatches_out, P.nmatches, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    }
-    ORB_CUDA(cudaStreamSynchronize(h->stream));
-    if (nmatches_out && nq == 0) *nmatches_out = 0;
-    return ORB_OK;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
+    if ((s = launch_proj(h, P, 1, nq, nq)) != ORB_OK) return s;
+    return copy_out(c);
 }
 
 extern "C" orb_status orbf_is_in_frustum(orbx_handle* h, const orbm_camera* cam, const orbf_frustum_points* in, float viewing_cos_limit,
@@ -722,32 +671,20 @@ extern "C" orb_status orbf_is_in_frustum(orbx_handle* h, const orbm_camera* cam,
         P.tcw = stage_in(c, in->tcw, (size_t)nf * 3, dev); P.Ow = stage_in(c, in->Ow, (size_t)nf * 3, dev);
         P.xw = stage_in(c, in->world_pos, (size_t)np * 3, dev); P.normal = stage_in(c, in->normal, (size_t)np * 3, dev);
         P.maxD = stage_in(c, in->max_dist, np, dev); P.minD = stage_in(c, in->min_dist, np, dev);
-        P.in_view = dev ? in_view_out : c.take<uint8_t>(np);
-        P.px = dev ? proj_x_out : c.take<float>(np);
-        P.py = dev ? proj_y_out : c.take<float>(np);
-        P.pxr = dev ? proj_xr_out : c.take<float>(np);
-        P.vc = dev ? view_cos_out : c.take<float>(np);
-        P.depth = dev ? track_depth_out : c.take<float>(np);
-        P.level = dev ? level_out : c.take<int>(np);
+        P.in_view = stage_out(c, in_view_out, np, dev);
+        P.px = stage_out(c, proj_x_out, np, dev);
+        P.py = stage_out(c, proj_y_out, np, dev);
+        P.pxr = stage_out(c, proj_xr_out, np, dev);
+        P.vc = stage_out(c, view_cos_out, np, dev);
+        P.depth = stage_out(c, track_depth_out, np, dev);
+        P.level = stage_out(c, level_out, np, dev);
     };
-    orb_status s;
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
     if (maxp > 0) {
         k_in_frustum<<<dim3((maxp + 255) / 256, nf), 256, 0, h->stream>>>(P);
         ORB_LAUNCHED();
         ORB_CUDA(cudaGetLastError());
     }
-    if (!dev) {
-        if (np > 0) {
-            ORB_CUDA(cudaMemcpyAsync(in_view_out, P.in_view, (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-            ORB_CUDA(cudaMemcpyAsync(proj_x_out, P.px, sizeof(float) * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-            ORB_CUDA(cudaMemcpyAsync(proj_y_out, P.py, sizeof(float) * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-            ORB_CUDA(cudaMemcpyAsync(proj_xr_out, P.pxr, sizeof(float) * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-            ORB_CUDA(cudaMemcpyAsync(level_out, P.level, sizeof(int) * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-            ORB_CUDA(cudaMemcpyAsync(view_cos_out, P.vc, sizeof(float) * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-            ORB_CUDA(cudaMemcpyAsync(track_depth_out, P.depth, sizeof(float) * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-        }
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-    }
-    return ORB_OK;
+    return dev ? ORB_OK : copy_out(c);
 }

@@ -374,24 +374,17 @@ extern "C" orb_status orbo_pose_optimization(orbx_handle* h, const orbo_pose_pro
         P.eoff = stage_in(c, in->edge_offset, nf + 1, dev); P.pose = stage_in(c, in->pose, (size_t)nf * 7, dev);
         P.xw = stage_in(c, in->world_pos, (size_t)ne * 3, dev); P.obs = stage_in(c, in->obs, (size_t)ne * 3, dev);
         P.invs2 = stage_in(c, in->inv_sigma2, ne, dev);
-        P.outlier = dev ? outlier_out : c.take<uint8_t>(ne);
-        P.pose_out = dev ? pose_out : c.take<double>((size_t)nf * 7);
-        P.inliers = dev ? inliers_out : c.take<int>(nf);
-        P.stats = (dev && stats_out) ? stats_out : c.take<int>((size_t)nf * 4);
+        P.outlier = stage_out(c, outlier_out, ne, dev);
+        P.pose_out = stage_out(c, pose_out, (size_t)nf * 7, dev);
+        P.inliers = stage_out(c, inliers_out, nf, dev);
+        P.stats = stage_out(c, stats_out, (size_t)nf * 4, dev);
     };
-    const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
-    if (s != ORB_OK) return s;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
     k_pose_opt<<<nf, PO_THREADS, 0, h->stream>>>(P);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
-    if (!dev) {
-        ORB_CUDA(cudaMemcpyAsync(pose_out, P.pose_out, sizeof(double) * 7 * (size_t)nf, cudaMemcpyDeviceToHost, h->stream));
-        if (ne > 0) ORB_CUDA(cudaMemcpyAsync(outlier_out, P.outlier, (size_t)ne, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaMemcpyAsync(inliers_out, P.inliers, sizeof(int) * (size_t)nf, cudaMemcpyDeviceToHost, h->stream));
-        if (stats_out) ORB_CUDA(cudaMemcpyAsync(stats_out, P.stats, sizeof(int) * 4 * (size_t)nf, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
-    }
-    return ORB_OK;
+    return dev ? ORB_OK : copy_out(c);
 }
 
 extern "C" orb_status orbo_pose_edges(orbx_handle* h, const orbo_edge_source* src, int32_t* edge_offset_out, int32_t* edge_feature_out,
@@ -410,7 +403,7 @@ extern "C" orb_status orbo_pose_edges(orbx_handle* h, const orbo_edge_source* sr
     P.xw = src->world_pos;
     P.xw2 = src->query_world_pos;
     for (int l = 0; l < ORB_MAX_LEVELS; ++l) P.invSigma2[l] = l < h->cfg.n_levels ? h->inv_sigma2[l] : 1.f;
-    const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, [&](Carve& c) { P.cnt = c.take<int>(nf); });
+    const orb_status s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, [&](Carve& c) { P.cnt = c.take<int>(nf); }).status;
     if (s != ORB_OK) return s;
     P.eoff = edge_offset_out; P.efeat = edge_feature_out; P.exw = world_pos_out; P.eobs = obs_out; P.ew = inv_sigma2_out;
     // one int per row of the handle: past 12 276 rows (48 KB less the 48 B of static arrays) the launch needs more than the default
@@ -449,29 +442,28 @@ extern "C" orb_status orbo_pose_optimization_frames(orbx_handle* h, const orbo_f
     cudaStream_t st = h->stream;
     orbo_edge_source src{nf};
     int *d_eoff, *d_efeat, *d_inl; float *d_pose, *d_exw, *d_eobs, *d_ew; double* d_pout; uint8_t* d_out;
+    std::vector<int> eoff(nf + 1), efeat(cap);    // the edge walk, read back only to scatter the outlier flags
+    std::vector<uint8_t> outl(cap);
+    const bool scatter = feature_outlier_out != nullptr;
     auto layout = [&](Carve& c) {
         src.frame_image = stage_in(c, in->frame_image, nf, false); d_pose = stage_in(c, in->pose, (size_t)nf * 7, false);
         src.world_pos = stage_in(c, in->world_pos, (size_t)nq * 3, false);
         src.feature_match = stage_in(c, in->feature_match, total_rows, false);
         if (in->query_match) { src.query_offset = stage_in(c, in->query_offset, nf + 1, false); src.query_match = stage_in(c, in->query_match, nqm, false); }
-        d_eoff = c.take<int>(nf + 1); d_efeat = c.take<int>(cap); d_exw = c.take<float>(cap * 3); d_eobs = c.take<float>(cap * 3);
-        d_ew = c.take<float>(cap); d_pout = c.take<double>((size_t)nf * 7); d_out = c.take<uint8_t>(cap); d_inl = c.take<int>(nf);
+        d_eoff = stage_out(c, scatter ? eoff.data() : nullptr, nf + 1, false);
+        d_efeat = stage_out(c, scatter ? efeat.data() : nullptr, cap, false);
+        d_exw = c.take<float>(cap * 3); d_eobs = c.take<float>(cap * 3); d_ew = c.take<float>(cap);
+        d_pout = stage_out(c, pose_out, (size_t)nf * 7, false);
+        d_out = stage_out(c, scatter ? outl.data() : nullptr, cap, false);
+        d_inl = stage_out(c, inliers_out, nf, false);
     };
-    if ((s = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout)) != ORB_OK) return s;
+    const Carve c = carve_scratch(h->po_bytes, h->d_po, h->capturing, st, layout);
+    if (c.status != ORB_OK) return c.status;
     if ((s = orbo_pose_edges(h, &src, d_eoff, d_efeat, d_exw, d_eobs, d_ew)) != ORB_OK) return s;
     orbo_pose_problems pp{nf, 1, d_eoff, d_pose, d_exw, d_eobs, d_ew, in->fx, in->fy, in->cx, in->cy, in->bf, (int32_t)cap};
     if ((s = orbo_pose_optimization(h, &pp, d_pout, d_out, d_inl, nullptr)) != ORB_OK) return s;
-    std::vector<int> eoff(nf + 1), efeat(cap);
-    std::vector<uint8_t> outl(cap);
-    ORB_CUDA(cudaMemcpyAsync(pose_out, d_pout, sizeof(double) * 7 * (size_t)nf, cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaMemcpyAsync(inliers_out, d_inl, sizeof(int) * (size_t)nf, cudaMemcpyDeviceToHost, st));
-    if (feature_outlier_out) {
-        ORB_CUDA(cudaMemcpyAsync(eoff.data(), d_eoff, sizeof(int) * (size_t)(nf + 1), cudaMemcpyDeviceToHost, st));
-        ORB_CUDA(cudaMemcpyAsync(efeat.data(), d_efeat, sizeof(int) * cap, cudaMemcpyDeviceToHost, st));
-        ORB_CUDA(cudaMemcpyAsync(outl.data(), d_out, cap, cudaMemcpyDeviceToHost, st));
-    }
-    ORB_CUDA(cudaStreamSynchronize(st));
-    if (feature_outlier_out) {                     // pFrame->mvbOutlier[i] of every feature of the listed frames
+    if ((s = copy_out(c)) != ORB_OK) return s;
+    if (scatter) {                     // pFrame->mvbOutlier[i] of every feature of the listed frames
         for (int f = 0; f < nf; ++f) {
             const int img = in->frame_image[f], row0 = h->h_counts[2 * MB + img];
             std::fill(feature_outlier_out + row0, feature_outlier_out + row0 + h->h_counts[img], (uint8_t)0);

@@ -198,7 +198,7 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         r->d_cview = c.take<uint8_t>(npK); r->d_cpx = c.take<float>(npK); r->d_cpy = c.take<float>(npK); r->d_cpxr = c.take<float>(npK);
         r->d_clevel = c.take<int>(npK); r->d_cvc = c.take<float>(npK); r->d_cdepth = c.take<float>(npK); r->d_posef = c.take<float>((size_t)nf * 7);
     };
-    orb_status s = carve_scratch(r->bytes, r->d_buf, h->capturing, h->stream, layout);
+    orb_status s = carve_scratch(r->bytes, r->d_buf, h->capturing, h->stream, layout).status;
     if (s != ORB_OK) return s;
     if (r->h_eoff_cap < 2 * (nf + 1)) {
         if (r->h_eoff) cudaFreeHost(r->h_eoff);

@@ -1,8 +1,14 @@
-// scratch.h -- per-call device scratch: one carver, one growth policy, one host-to-device staging helper (host code only)
+// scratch.h -- per-call device scratch: one carver, one growth policy, one staging helper for each direction (host code only)
 //
 // An entry point describes its scratch block once, as a `layout` function of a Carve that assigns every device pointer.
 // carve_scratch runs it with a null base to measure, grows the buffer to fit and runs it again on the buffer, so the size
 // always matches what the layout takes.
+//
+// Arrays an entry point takes in or returns name the caller's pointer once in the layout.  stage_in gives a device caller its own
+// pointer back and copies a host array into a slot of the block.  stage_out gives a device caller its own pointer back and gives a
+// host caller a slot whose contents copy_out later copies to the caller's array; an in-out array is staged in and then named in
+// a copy_back.  copy_out issues every recorded copy and waits for the stream, so a host-form call ends with it and a device-form
+// call, which records none, never calls it.
 //
 // Some calls nest, so a call never carves the arena its caller carves.  Which entry points use which buffer:
 //
@@ -28,7 +34,11 @@ struct Carve {
     uint8_t* base;               // nullptr: measure only
     cudaStream_t stream = nullptr;
     size_t off = 0;
-    orb_status status = ORB_OK;  // first failed copy of stage_in
+    orb_status status = ORB_OK;  // first failed copy of stage_in, or a copy_back past kMaxOut
+    struct Out { void* dst; const void* src; size_t bytes; };
+    static constexpr int kMaxOut = 8;   // the most results one entry point returns (orbf_is_in_frustum: 7)
+    Out out[kMaxOut] = {};
+    int n_out = 0;
     // 256-byte aligned; at least one element, so no two arrays share an address
     template <typename T>
     T* take(size_t n) {
@@ -36,6 +46,16 @@ struct Carve {
         T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
         off += std::max<size_t>(n, 1) * sizeof(T);
         return p;
+    }
+    // records a device-to-host copy of n elements for copy_out; nothing on the measuring pass or for a null dst
+    template <typename T>
+    void copy_back(T* dst, const T* src, size_t n) {
+        if (!base || !dst) return;
+        if (n_out == kMaxOut) {
+            status = set_error(ORB_ERR_CAPACITY, "copy_back: more than Carve::kMaxOut results");
+            return;
+        }
+        out[n_out++] = {dst, src, n * sizeof(T)};
     }
 };
 
@@ -50,6 +70,24 @@ T* stage_in(Carve& c, const T* src, size_t n, bool on_device) {
         if (e != cudaSuccess) c.status = set_error(ORB_ERR_CUDA, std::string("stage_in: cudaMemcpyAsync -> ") + cudaGetErrorString(e));
     }
     return dst;
+}
+
+// Device callers get their own pointer back; host arrays get a slot in the block, copied back by copy_out.  A null dst (an optional
+// result the caller did not ask for) still gets a slot, since the kernels write it.
+template <typename T>
+T* stage_out(Carve& c, T* dst, size_t n, bool on_device) {
+    if (on_device && dst) return dst;
+    T* p = c.take<T>(n);
+    if (!on_device) c.copy_back(dst, p, n);
+    return p;
+}
+
+// Issues the copies the layout recorded, in order, and waits for the stream: returns the first error.
+inline orb_status copy_out(const Carve& c) {
+    for (int i = 0; i < c.n_out; ++i)
+        if (c.out[i].bytes) ORB_CUDA(cudaMemcpyAsync(c.out[i].dst, c.out[i].src, c.out[i].bytes, cudaMemcpyDeviceToHost, c.stream));
+    ORB_CUDA(cudaStreamSynchronize(c.stream));
+    return ORB_OK;
 }
 
 // Grow only, never shrink.  A quarter of headroom keeps calls whose sizes vary a little from reallocating every time.
@@ -124,16 +162,20 @@ inline void solver_release(SolverHandle* h) {
     if (h->stream) cudaStreamDestroy(h->stream);
 }
 
-// measure `layout`, grow the buffer to fit, carve it: returns the first error of the growth or of a stage_in copy
+// measure `layout`, grow the buffer to fit, carve it: returns the filled carve (its copies for copy_out), whose status is the first
+// error of the growth, of a stage_in copy or of a copy_back
 template <typename F>
-orb_status carve_scratch(size_t& bytes, uint8_t*& ptr, bool capturing, cudaStream_t stream, F&& layout) {
+Carve carve_scratch(size_t& bytes, uint8_t*& ptr, bool capturing, cudaStream_t stream, F&& layout) {
     Carve m{nullptr, stream};
     layout(m);
     const orb_status s = grow_device(bytes, ptr, m.off, capturing);
-    if (s != ORB_OK) return s;
+    if (s != ORB_OK) {
+        m.status = s;
+        return m;
+    }
     Carve c{ptr, stream};
     layout(c);
-    return c.status;
+    return c;
 }
 
 }  // namespace orb

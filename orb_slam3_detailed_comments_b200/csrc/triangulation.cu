@@ -184,21 +184,17 @@ extern "C" orb_status orbm_search_triangulation(orbx_handle* h, const orbm_trian
         P.node1 = stage_in(c, T->node1, nq, false); P.stereo1 = stage_in(c, T->stereo1, nq, false);
         P.kp2 = stage_in(c, T->kp2, N2, false); P.desc2 = stage_in(c, T->desc2, (size_t)N2 * 32, false);
         P.node2 = stage_in(c, T->node2, N2, false); P.valid2 = stage_in(c, T->valid2, N2, false); P.stereo2 = stage_in(c, T->stereo2, N2, false);
-        P.match = c.take<int>(nq);
+        P.match = stage_out(c, match12_out, nq, false);
         P.bins = c.take<int>(nq);
-        P.nmatches = c.take<int>(1);
+        P.nmatches = stage_out(c, nmatches_out, 1, false);
     };
-    if ((s = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout)) != ORB_OK) return s;
+    const Carve c = carve_scratch(h->stage_bytes, h->d_stage, h->capturing, h->stream, layout);
+    if (c.status != ORB_OK) return c.status;
     ORB_CUDA(cudaFuncSetAttribute(k_tri_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem, (size_t)1024)));
     k_tri_match<<<(nq + TRI_QPB - 1) / TRI_QPB, TRI_WARPS * 32, smem, h->stream>>>(P);
     ORB_LAUNCHED();
     k_tri_rotation<<<1, 256, 0, h->stream>>>(P);
     ORB_LAUNCHED();
     ORB_CUDA(cudaGetLastError());
-    int nm = 0;
-    ORB_CUDA(cudaMemcpyAsync(match12_out, P.match, (size_t)nq * 4, cudaMemcpyDeviceToHost, h->stream));
-    ORB_CUDA(cudaMemcpyAsync(&nm, P.nmatches, 4, cudaMemcpyDeviceToHost, h->stream));
-    ORB_CUDA(cudaStreamSynchronize(h->stream));
-    if (nmatches_out) *nmatches_out = nm;
-    return ORB_OK;
+    return copy_out(c);
 }
