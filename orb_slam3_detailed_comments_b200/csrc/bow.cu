@@ -16,6 +16,7 @@ using namespace orb;
 struct orbv_vocabulary {
     int device = 0;
     int n_nodes = 0, L = 0, max_children = 0;
+    uint8_t* d_buf = nullptr;   // the five arrays below, carved from one block
     int* d_child_off = nullptr;
     int* d_child = nullptr;
     uint8_t* d_desc = nullptr;
@@ -139,16 +140,16 @@ extern "C" orb_status orbv_create(int32_t device, int32_t n_nodes, int32_t depth
     orbv_vocabulary* v = new orbv_vocabulary();
     v->device = device; v->n_nodes = n_nodes; v->L = depth_levels;
     for (int i = 0; i < n_nodes; ++i) v->max_children = std::max(v->max_children, child_offset[i + 1] - child_offset[i]);
-    auto up = [&](auto*& dst, const auto* src, size_t n) -> orb_status {
-        using T = std::remove_cv_t<std::remove_pointer_t<decltype(src)>>;
-        ORB_CUDA(cudaMalloc((void**)&dst, std::max<size_t>(n, 1) * sizeof(T)));
-        ORB_CUDA(cudaMemcpy(dst, src, n * sizeof(T), cudaMemcpyHostToDevice));
-        return ORB_OK;
+    auto layout = [&](Carve& c) {
+        v->d_child_off = stage_in(c, child_offset, (size_t)n_nodes + 1, false);
+        v->d_child = stage_in(c, child_ids, (size_t)nchild, false);
+        v->d_desc = stage_in(c, node_desc, (size_t)n_nodes * 32, false);
+        v->d_word = stage_in(c, node_word, (size_t)n_nodes, false);
+        v->d_weight = stage_in(c, node_weight, (size_t)n_nodes, false);
     };
-    orb_status s;
-    if ((s = up(v->d_child_off, (const int*)child_offset, (size_t)n_nodes + 1)) != ORB_OK || (s = up(v->d_child, (const int*)child_ids, (size_t)nchild)) != ORB_OK ||
-        (s = up(v->d_desc, node_desc, (size_t)n_nodes * 32)) != ORB_OK || (s = up(v->d_word, (const int*)node_word, (size_t)n_nodes)) != ORB_OK ||
-        (s = up(v->d_weight, node_weight, (size_t)n_nodes)) != ORB_OK) {
+    orb_status s = carve_exact(v->d_buf, nullptr, layout).status;
+    if (s == ORB_OK && cudaStreamSynchronize(nullptr) != cudaSuccess) s = set_error(ORB_ERR_CUDA, "vocabulary upload failed");
+    if (s != ORB_OK) {
         orbv_destroy(v);
         return s;
     }
@@ -159,9 +160,7 @@ extern "C" orb_status orbv_create(int32_t device, int32_t n_nodes, int32_t depth
 extern "C" void orbv_destroy(orbv_vocabulary* v) {
     if (!v) return;
     cudaSetDevice(v->device);
-    void* ptrs[] = {v->d_child_off, v->d_child, v->d_desc, v->d_word, v->d_weight};
-    for (void* p : ptrs)
-        if (p) cudaFree(p);
+    if (v->d_buf) cudaFree(v->d_buf);
     delete v;
 }
 

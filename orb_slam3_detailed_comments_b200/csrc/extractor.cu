@@ -198,15 +198,20 @@ static orb_status plan_geometry(orbx_handle* h, int w, int hh) {
     return ORB_OK;
 }
 
-static size_t level_bytes_total(const orbx_handle* h, int w, int hh) {
-    size_t off = 0;
+// Places the levels of the planned geometry in the two pyramid blocks, each level base 256-byte aligned (the ORB_FAST_TMA path needs
+// 16): returns the bytes the levels take.  On null blocks (orbx_create's sizing) it only measures.
+static size_t place_levels(orbx_handle* h) {
+    Carve pyr{h->d_pyr}, blur{h->d_blur};
     for (int l = 0; l < h->cfg.n_levels; ++l) {
-        const int lw = (int)lrintf((float)w * h->inv_scale[l]), lh = (int)lrintf((float)hh * h->inv_scale[l]);
-        off += (size_t)round_up(lw, 16) * lh * h->cfg.max_batch;
-        off = (off + 255) / 256 * 256;
+        LevelGeom& L = h->geom.lv[l];
+        L.base = pyr.take<uint8_t>((size_t)L.img_stride * h->cfg.max_batch);
+        L.blur = blur.take<uint8_t>((size_t)L.img_stride * h->cfg.max_batch);
     }
-    return off;
+    return (pyr.off + 255) / 256 * 256;
 }
+
+// One (image, level)'s quadtree node workspace: qt_node_cap(N) nodes for the largest quota N (quadtree_core.cuh)
+static size_t qt_node_bytes(const orbx_handle* h) { return (qt_work_bytes(h->qt_node_cap) + 15) / 16 * 16; }
 
 extern "C" const char* orb_last_error(void) { return g_last_error.c_str(); }
 extern "C" int orb_device_count(void) {
@@ -236,45 +241,15 @@ static orb_status apply_geometry(orbx_handle* h, int w, int hh) {
         h->cur_w = h->cur_h = -1;
         return s;
     }
-    // fix the level base pointers (plan_geometry used running offsets)
-    size_t off = 0;
-    for (int l = 0; l < h->cfg.n_levels; ++l) {
-        LevelGeom& L = h->geom.lv[l];
-        L.base = h->d_pyr + off;
-        L.blur = h->d_blur + off;
-        off += (size_t)L.img_stride * h->cfg.max_batch;
-        off = (off + 255) / 256 * 256;
-    }
-    if (off > h->pyr_bytes) return set_error(ORB_ERR_CAPACITY, "pyramid allocation too small");
+    if (place_levels(h) + 4096 > h->pyr_bytes) return set_error(ORB_ERR_CAPACITY, "pyramid allocation too small");
     if ((size_t)h->geom.candTotal > h->cand_slots || (size_t)h->geom.kpTotal > h->kp_slots ||
-        (size_t)h->geom.sortTotal > h->sort_slots || h->taps_host.size() > h->taps_slots)
+        (size_t)h->geom.sortTotal > h->sort_slots || h->taps_host.size() > h->taps_slots || h->cells_host.size() > h->cells_slots)
         return set_error(ORB_ERR_CAPACITY, "workspace sized for max image is too small for this size");
     ORB_CUDA(cudaMemcpyAsync(h->d_taps, h->taps_host.data(), h->taps_host.size() * sizeof(int2), cudaMemcpyHostToDevice,
                              h->stream));
-    if (h->cells_host.size() > h->cells_slots) {
-        if (h->d_cells) cudaFree(h->d_cells);
-        h->d_cells = nullptr;
-        h->cells_slots = h->cells_host.size() + 64;
-        ORB_CUDA(cudaMalloc(&h->d_cells, h->cells_slots * sizeof(uint2)));
-    }
     ORB_CUDA(cudaMemcpyAsync(h->d_cells, h->cells_host.data(), h->cells_host.size() * sizeof(uint2), cudaMemcpyHostToDevice, h->stream));
     ORB_CUDA(cudaStreamSynchronize(h->stream));
-    // quadtree launch plan.  Node workspace: qt_node_cap(N) nodes (N + 20, see quadtree_core.cuh).
-    int capMax = 0;
-    for (int l = 0; l < h->cfg.n_levels; ++l) capMax = std::max(capMax, qt_node_cap(h->geom.lv[l].quota));
-    h->qt_node_cap = capMax;
-    const size_t nodeBytes = (qt_work_bytes(capMax) + 15) / 16 * 16;
-    h->qt_nodes_in_smem = nodeBytes <= 96 * 1024 ? 1 : 0;
-    h->qt_node_stride = (nodeBytes + 255) / 256 * 256;
-    if (!h->qt_nodes_in_smem) {
-        const size_t need = h->qt_node_stride * (size_t)h->cfg.max_batch * h->cfg.n_levels;
-        if (need > h->node_scratch_bytes) {
-            if (h->d_node_scratch) cudaFree(h->d_node_scratch);
-            h->d_node_scratch = nullptr;
-            ORB_CUDA(cudaMalloc(&h->d_node_scratch, need));
-            h->node_scratch_bytes = need;
-        }
-    }
+    const size_t nodeBytes = qt_node_bytes(h);
     // Sort capacity in shared memory per level: a texture-rich level yields about one FAST candidate
     // per 37 tested pixels; provision area/24 and fall back to the global scratch beyond that.
     // Consecutive levels with the same capacity form a group (<= 4 groups, one launch each on its own stream).
@@ -381,63 +356,61 @@ extern "C" orb_status orbx_create(const orbx_config* cfg, orbx_handle** out) {
         cudaEventCreateWithFlags(&h->ev_join[i], cudaEventDisableTiming);
     }
     cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming);
-    // size every buffer for the largest image
-    h->pyr_bytes = level_bytes_total(h, cfg->max_width, cfg->max_height) + 4096;
-    h->cur_w = h->cur_h = -1;
-    // dry geometry pass for capacities (base pointers are null; only sizes are read)
+    // size every buffer for the largest image: the capacities of the max-size plan bound every size the handle accepts
     h->d_pyr = h->d_blur = nullptr;
     s = plan_geometry(h, cfg->max_width, cfg->max_height);
     if (s != ORB_OK) return fail(s);
     h->cur_w = h->cur_h = -1;
     const int B = cfg->max_batch;
+    h->pyr_bytes = place_levels(h) + 4096;   // slack after the last level: k_resize_v3 reads own levels up to d_pyr + pyr_bytes
     h->cand_slots = h->geom.candTotal + 64;
     h->kp_slots = h->geom.kpTotal + 64;
     h->sort_slots = h->geom.sortTotal + 64;
     h->taps_slots = h->taps_host.size() + 4 * (cfg->max_width + cfg->max_height) + 64;
+    h->cells_slots = h->geom.totalCells;   // monotone in the image's width and height
     h->out_rows = (size_t)h->kp_slots * B;
-#define ALLOC(ptr, bytes)                                                                        \
-    if (cudaMalloc((void**)&(ptr), (bytes)) != cudaSuccess)                                      \
-        return fail(set_error(ORB_ERR_CUDA, std::string("cudaMalloc failed: ") + #ptr));
-    ALLOC(h->d_pyr, h->pyr_bytes);
-    ALLOC(h->d_blur, h->pyr_bytes);
-    ALLOC(h->d_cand, h->cand_slots * 4 * B);
-    ALLOC(h->d_sort, h->sort_slots * 4 * B);
-    ALLOC(h->d_lvl_kp, h->kp_slots * 4 * B);
-    ALLOC(h->d_slot, h->kp_slots * 4 * B);
-    ALLOC(h->d_cand_cnt, sizeof(int) * B * ORB_MAX_LEVELS);
-    ALLOC(h->d_lvl_cnt, sizeof(int) * B * ORB_MAX_LEVELS);
-    ALLOC(h->d_nkp, sizeof(int) * (3 * B + 8));
-    ALLOC(h->d_err, sizeof(int) * 8);
-    ALLOC(h->d_taps, h->taps_slots * sizeof(int2));
-    ALLOC(h->d_kps, h->out_rows * sizeof(orbx_keypoint));
-    ALLOC(h->d_desc, h->out_rows * 32);
-    ALLOC(h->d_uright, h->out_rows * sizeof(float));
-    ALLOC(h->d_depth, h->out_rows * sizeof(float));
-    ALLOC(h->d_sad, h->out_rows * sizeof(int));
-    ALLOC(h->d_pat, 256 * sizeof(uint32_t));
-    ALLOC(h->d_blur_frag, 256 * sizeof(uint32_t));
-#undef ALLOC
-    {
-        uint32_t frag[256];
-        orbdev::bm_fragments(frag);
-        if (cudaMemcpy(h->d_blur_frag, frag, sizeof(frag), cudaMemcpyHostToDevice) != cudaSuccess)
-            return fail(set_error(ORB_ERR_CUDA, "blur fragment upload failed"));
-    }
+    // the quadtree node workspace depends on the quotas only: in shared memory when it fits, else one block per (image, level)
+    for (int l = 0; l < cfg->n_levels; ++l) h->qt_node_cap = std::max(h->qt_node_cap, qt_node_cap(h->quota[l]));
+    h->qt_nodes_in_smem = qt_node_bytes(h) <= 96 * 1024 ? 1 : 0;
+    h->qt_node_stride = (qt_node_bytes(h) + 255) / 256 * 256;
+    uint32_t frag[256], pat_w[256];
+    orbdev::bm_fragments(frag);
     {   // the rBRIEF pattern as 256 packed words (xa, ya, xb, yb), transposed to [pair % 8][pair / 8] for k_orient_describe
         static const int8_t pat[1024] = {
 #include "orb_pattern.inc"
         };
-        uint32_t w[256];
         for (int i = 0; i < 256; ++i)
-            w[(i & 7) * 32 + (i >> 3)] = (uint32_t)(uint8_t)pat[4 * i] | ((uint32_t)(uint8_t)pat[4 * i + 1] << 8) | ((uint32_t)(uint8_t)pat[4 * i + 2] << 16) |
-                                         ((uint32_t)(uint8_t)pat[4 * i + 3] << 24);
-        if (cudaMemcpy(h->d_pat, w, sizeof(w), cudaMemcpyHostToDevice) != cudaSuccess) return fail(set_error(ORB_ERR_CUDA, "pattern upload failed"));
+            pat_w[(i & 7) * 32 + (i >> 3)] = (uint32_t)(uint8_t)pat[4 * i] | ((uint32_t)(uint8_t)pat[4 * i + 1] << 8) |
+                                             ((uint32_t)(uint8_t)pat[4 * i + 2] << 16) | ((uint32_t)(uint8_t)pat[4 * i + 3] << 24);
     }
+    auto layout = [&](Carve& c) {
+        h->d_pyr = c.take<uint8_t>(h->pyr_bytes);
+        h->d_blur = c.take<uint8_t>(h->pyr_bytes);
+        h->d_cand = c.take<uint32_t>(h->cand_slots * B);
+        h->d_sort = c.take<uint32_t>(h->sort_slots * B);
+        h->d_lvl_kp = c.take<uint32_t>(h->kp_slots * B);
+        h->d_slot = c.take<int>(h->kp_slots * B);
+        h->d_cand_cnt = c.take<int>((size_t)B * ORB_MAX_LEVELS);
+        h->d_lvl_cnt = c.take<int>((size_t)B * ORB_MAX_LEVELS);
+        h->d_nkp = c.take<int>(3 * B + 8);
+        h->d_err = c.take<int>(8);
+        h->d_taps = c.take<int2>(h->taps_slots);
+        h->d_kps = c.take<orbx_keypoint>(h->out_rows);
+        h->d_desc = c.take<uint8_t>(h->out_rows * 32);
+        h->d_uright = c.take<float>(h->out_rows);
+        h->d_depth = c.take<float>(h->out_rows);
+        h->d_sad = c.take<int>(h->out_rows);
+        h->d_pat = stage_in(c, pat_w, 256, false);
+        h->d_blur_frag = stage_in(c, frag, 256, false);
+        h->d_cells = c.take<uint2>(h->cells_slots);
+        if (!h->qt_nodes_in_smem) h->d_node_scratch = c.take<uint8_t>(h->qt_node_stride * B * cfg->n_levels);
+    };
+    if ((s = carve_exact(h->d_ws, h->stream, layout).status) != ORB_OK) return fail(s);
     h->d_mono = h->d_nkp + B;
     h->d_offsets = h->d_nkp + 2 * B;
-    cudaMemset(h->d_err, 0, sizeof(int) * 8);
-    cudaMemset(h->d_pyr, 0, h->pyr_bytes);
-    cudaMemset(h->d_blur, 0, h->pyr_bytes);
+    cudaMemsetAsync(h->d_err, 0, sizeof(int) * 8, h->stream);
+    cudaMemsetAsync(h->d_pyr, 0, h->pyr_bytes, h->stream);
+    cudaMemsetAsync(h->d_blur, 0, h->pyr_bytes, h->stream);
     if (cudaMallocHost((void**)&h->h_counts, sizeof(int) * (3 * B + 16)) != cudaSuccess)
         return fail(set_error(ORB_ERR_CUDA, "cudaMallocHost failed"));
     s = apply_geometry(h, cfg->max_width, cfg->max_height);
@@ -451,10 +424,7 @@ extern "C" void orbx_destroy(orbx_handle* h) {
     cudaSetDevice(h->cfg.device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     orbr_release(h);
-    void* ptrs[] = {h->d_pyr, h->d_blur, h->d_cand, h->d_sort, h->d_lvl_kp, h->d_slot, h->d_cand_cnt, h->d_lvl_cnt,
-                    h->d_nkp, h->d_err, h->d_taps, h->d_kps, h->d_desc, h->d_node_scratch, h->d_stage, h->d_po,
-                    h->d_uright, h->d_depth, h->d_sad, h->d_cells, h->d_pat, h->d_blur_frag, h->d_xl};
-    for (void* p : ptrs)
+    for (void* p : {h->d_ws, h->d_stage, h->d_po, h->d_xl})
         if (p) cudaFree(p);
     if (h->h_counts) cudaFreeHost(h->h_counts);
     for (int r = 0; r < orbx_handle::kProfRing; ++r)
@@ -654,32 +624,51 @@ extern "C" orb_status orbx_extract_batch(orbx_handle* h, const uint8_t* imgs, in
     return s;
 }
 
-extern "C" orb_status orbx_counts(orbx_handle* h, int32_t* n, int32_t* mono_index, int32_t* offsets) {
-    if (!h || h->last_batch < 1) return set_error(ORB_ERR_INVALID, "no batch has been extracted");
-    const int B = h->last_batch, MB = h->cfg.max_batch;
+// ---- the batch count table ------------------------------------------------------------------------------------------------
+// d_nkp holds [max_batch] features per image (k_order), [max_batch] mono indices (k_order) and [max_batch + 1] first rows
+// (k_offsets).  h_counts mirrors those words, then holds the first four words of d_err at 3 max_batch + 4: [0] FAST candidate
+// overflow, [1] quadtree node overflow.
+orb_status queue_counts(orbx_handle* h) {
+    const int MB = h->cfg.max_batch;
+    ORB_CUDA(cudaMemcpyAsync(h->h_counts, h->d_nkp, sizeof(int) * (3 * MB + 1), cudaMemcpyDeviceToHost, h->stream));
+    ORB_CUDA(cudaMemcpyAsync(h->h_counts + 3 * MB + 4, h->d_err, sizeof(int) * 4, cudaMemcpyDeviceToHost, h->stream));
+    return ORB_OK;
+}
+
+orb_status latch_counts(orbx_handle* h) {
     if (!h->counts_valid) {
-        ORB_CUDA(cudaMemcpyAsync(h->h_counts, h->d_nkp, sizeof(int) * (3 * MB + 1), cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaMemcpyAsync(h->h_counts + 3 * MB + 4, h->d_err, sizeof(int) * 4, cudaMemcpyDeviceToHost, h->stream));
-        ORB_CUDA(cudaStreamSynchronize(h->stream));
         h->counts_valid = true;
-        const int* e = h->h_counts + 3 * MB + 4;
+        const int* e = h->h_counts + 3 * h->cfg.max_batch + 4;
         h->batch_status = (e[0] || e[1]) ? (e[0] ? 1 : 2) : 0;   // latched until the next extract: every accessor keeps reporting it
         if (h->batch_status) cudaMemsetAsync(h->d_err, 0, sizeof(int) * 8, h->stream);
     }
     if (h->batch_status)
         return set_error(ORB_ERR_CAPACITY, h->batch_status == 1 ? "FAST candidate capacity exceeded" : "quadtree node capacity exceeded");
-    for (int b = 0; b < B; ++b) {
-        if (n) n[b] = h->h_counts[b];
-        if (mono_index) mono_index[b] = h->h_counts[MB + b];
-        if (offsets) offsets[b] = h->h_counts[2 * MB + b];
+    return ORB_OK;
+}
+
+extern "C" orb_status orbx_counts(orbx_handle* h, int32_t* n, int32_t* mono_index, int32_t* offsets) {
+    if (!h || h->last_batch < 1) return set_error(ORB_ERR_INVALID, "no batch has been extracted");
+    const int B = h->last_batch, MB = h->cfg.max_batch;
+    if (!h->counts_valid) {
+        orb_status s = queue_counts(h);
+        if (s != ORB_OK) return s;
+        ORB_CUDA(cudaStreamSynchronize(h->stream));
     }
-    if (offsets) offsets[B] = h->h_counts[2 * MB + B];
+    const orb_status s = latch_counts(h);
+    if (s != ORB_OK) return s;
+    for (int b = 0; b < B; ++b) {
+        if (n) n[b] = image_features(h, b);
+        if (mono_index) mono_index[b] = h->h_counts[MB + b];
+        if (offsets) offsets[b] = image_row0(h, b);
+    }
+    if (offsets) offsets[B] = image_row0(h, B);
     return ORB_OK;
 }
 
 orb_status batch_rows(orbx_handle* h, int* rows) {
     const orb_status s = orbx_counts(h, nullptr, nullptr, nullptr);
-    if (s == ORB_OK) *rows = h->h_counts[2 * h->cfg.max_batch + h->last_batch];
+    if (s == ORB_OK) *rows = batch_total_rows(h);
     return s;
 }
 

@@ -8,6 +8,9 @@
 struct orbr_state;
 void orbr_release(struct orbx_handle* h);   // replay.cu
 orb_status batch_rows(struct orbx_handle* h, int* rows);   // extractor.cu: compact rows of the last batch (orbx_counts)
+// The batch count table (extractor.cu): queue its read-back on the handle's stream; after the wait, latch its capacity flags
+orb_status queue_counts(struct orbx_handle* h);
+orb_status latch_counts(struct orbx_handle* h);
 
 struct orbx_handle {
     orbx_config cfg{};
@@ -16,7 +19,6 @@ struct orbx_handle {
     int fast_variant = 1; // 1 (default): k_fast_cells_v2; 0: the round-1 k_fast_cells (ORB_FAST_VARIANT=0 at orbx_create)
     std::vector<uint2> cells_host;   // k_fast_cells_v2: one record per non-empty FAST cell
     uint2* d_cells = nullptr;
-    size_t cells_slots = 0;
     int fast_R = 0, fast_PW = 0, fast_LW = 0;
     int blur_variant = 2;    // 2: k_blur_mma (both passes as u8 IMMA, default), 1: k_blur<true> (IDP.4A horizontal pass), 0: k_blur<false>
     int resize_variant = 1;  // 1: k_resize_v2 (default), 0: k_resize
@@ -32,7 +34,8 @@ struct orbx_handle {
     std::vector<float> scale, inv_scale, sigma2, inv_sigma2;
     std::vector<int> quota, umax;
     std::vector<int2> taps_host;
-    // device workspace (sized for max_width x max_height x max_batch)
+    // device workspace (sized for max_width x max_height x max_batch), carved from one block (orbx_create)
+    uint8_t* d_ws = nullptr;
     uint8_t* d_pyr = nullptr;      // level-major pyramids (mvImagePyramid)
     uint8_t* d_blur = nullptr;     // blurred pyramids
     size_t pyr_bytes = 0;
@@ -42,7 +45,7 @@ struct orbx_handle {
     int* d_slot = nullptr;         // output row of every emitted keypoint
     int* d_cand_cnt = nullptr;
     int* d_lvl_cnt = nullptr;
-    int* d_nkp = nullptr;          // [max_batch] n, [max_batch] mono, [max_batch+1] offsets
+    int* d_nkp = nullptr;          // the count table: [max_batch] n, [max_batch] mono, [max_batch+1] offsets
     int* d_mono = nullptr;
     int* d_offsets = nullptr;
     int* d_err = nullptr;
@@ -54,13 +57,13 @@ struct orbx_handle {
     int* d_sad = nullptr;
     uint32_t* d_pat = nullptr;       // rBRIEF pattern, 256 packed pairs transposed for k_orient_describe
     uint32_t* d_blur_frag = nullptr; // k_blur_mma: the lanes' constant A fragments (bm_fragments, 8 x 32 words)
-    void* d_node_scratch = nullptr;
+    uint8_t* d_node_scratch = nullptr;   // quadtree nodes when they do not fit shared memory (!qt_nodes_in_smem)
     uint8_t* d_stage = nullptr;
     uint8_t* d_po = nullptr;         // edge lists / results of orbo_pose_optimization_frames
-    size_t node_scratch_bytes = 0, stage_bytes = 0, po_bytes = 0;
+    size_t stage_bytes = 0, po_bytes = 0;
     bool stereo_valid = false;   // d_uright/d_depth belong to the last extracted batch
-    size_t cand_slots = 0, kp_slots = 0, sort_slots = 0, taps_slots = 0, out_rows = 0;
-    int* h_counts = nullptr;       // pinned
+    size_t cand_slots = 0, kp_slots = 0, sort_slots = 0, taps_slots = 0, cells_slots = 0, out_rows = 0;
+    int* h_counts = nullptr;       // pinned mirror of the count table, then the capacity flags (extractor.cu queue_counts)
     bool counts_valid = false;
     int q_total_bound = 0, q_frame_bound = 0, rows_bound = 0;   // orbm_set_device_query_bounds: sync-free device-pointer searches
     bool capturing = false;   // between orbx_graph_begin and orbx_graph_end
@@ -95,6 +98,11 @@ inline orb_status check_frame_rows(long long rows, const char* what) {
     return orb::set_error(ORB_ERR_UNSUPPORTED, std::string(what) + " with " + std::to_string(rows) + " feature rows: the matchers take at most " +
                                                    std::to_string(ORB_MAX_FRAME_ROWS));
 }
+
+// What the count table of the last batch says, once orbx_counts, batch_rows or orbr_collect has read it back
+inline int image_features(const orbx_handle* h, int img) { return h->h_counts[img]; }
+inline int image_row0(const orbx_handle* h, int img) { return h->h_counts[2 * h->cfg.max_batch + img]; }
+inline int batch_total_rows(const orbx_handle* h) { return image_row0(h, h->last_batch); }
 
 inline int smem_optin(orbx_handle* h) {
     if (h->smem_optin == 0) cudaDeviceGetAttribute(&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->cfg.device);

@@ -355,6 +355,8 @@ extern "C" orb_status orbm_search_local_points(orbx_handle* h, const orbm_camera
     int nq, maxq, rows;
     orb_status s = frame_table(h, nf, Q->frame_image, Q->query_offset, dev, bounded, nq, maxq, rows);
     if (s != ORB_OK) return s;
+    if (nq > 0 && (!Q->proj_x || !Q->proj_y || !Q->proj_xr || !Q->level || !Q->view_cos || !Q->desc))
+        return set_error(ORB_ERR_INVALID, "missing query arrays");
     ProjParams P{};
     fill_frame_side(h, cam, P);
     if ((s = check_frame_rows(P.maxFeat, "frame")) != ORB_OK) return s;
@@ -393,6 +395,7 @@ extern "C" orb_status orbm_search_last_frame(orbx_handle* h, const orbm_camera* 
     int nq, maxq, total_rows;
     orb_status s = frame_table(h, nf, Q->frame_image, Q->query_offset, dev, bounded, nq, maxq, total_rows);
     if (s != ORB_OK) return s;
+    if (nq > 0 && (!Q->world_pos || !Q->last_octave || !Q->last_angle || !Q->desc)) return set_error(ORB_ERR_INVALID, "missing query arrays");
     ProjParams P{};
     fill_frame_side(h, cam, P);
     if ((s = check_frame_rows(P.maxFeat, "frame")) != ORB_OK) return s;
@@ -431,6 +434,7 @@ extern "C" orb_status orbm_search_bow(orbx_handle* h, const orbm_bow_queries* Q,
     int nq, maxq, total_rows;
     orb_status s = frame_table(h, nf, Q->frame_image, Q->query_offset, dev, false, nq, maxq, total_rows);
     if (s != ORB_OK) return s;
+    if (nq > 0 && (!Q->query_node || !Q->query_angle || !Q->desc)) return set_error(ORB_ERR_INVALID, "missing query arrays");
     ProjParams P{};
     orbm_camera cam{1, 1, 0, 0, 0, 1, 0, (float)h->cur_w, 0, (float)h->cur_h};   // the grid is not used by this search
     fill_frame_side(h, &cam, P);

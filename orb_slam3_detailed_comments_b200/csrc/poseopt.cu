@@ -429,12 +429,12 @@ extern "C" orb_status orbo_pose_optimization_frames(orbx_handle* h, const orbo_f
     int total_rows = 0;
     orb_status s = batch_rows(h, &total_rows);
     if (s != ORB_OK) return s;
-    const int nf = in->n_frames, MB = h->cfg.max_batch;
+    const int nf = in->n_frames;
     size_t cap = 0;                               // edges <= features of the listed frames
     for (int f = 0; f < nf; ++f) {
         const int img = in->frame_image[f];
         if (img < 0 || img >= h->last_batch) return set_error(ORB_ERR_INVALID, "bad frame image");
-        cap += (size_t)h->h_counts[img];
+        cap += (size_t)image_features(h, img);
     }
     cap = std::max<size_t>(cap, 1);
     const int nq = in->n_queries;
@@ -465,8 +465,8 @@ extern "C" orb_status orbo_pose_optimization_frames(orbx_handle* h, const orbo_f
     if ((s = copy_out(c)) != ORB_OK) return s;
     if (scatter) {                     // pFrame->mvbOutlier[i] of every feature of the listed frames
         for (int f = 0; f < nf; ++f) {
-            const int img = in->frame_image[f], row0 = h->h_counts[2 * MB + img];
-            std::fill(feature_outlier_out + row0, feature_outlier_out + row0 + h->h_counts[img], (uint8_t)0);
+            const int img = in->frame_image[f], row0 = image_row0(h, img);
+            std::fill(feature_outlier_out + row0, feature_outlier_out + row0 + image_features(h, img), (uint8_t)0);
             for (int e = eoff[f]; e < eoff[f + 1]; ++e) feature_outlier_out[row0 + efeat[e]] = outl[e];
         }
     }

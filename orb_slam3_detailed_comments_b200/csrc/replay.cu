@@ -36,7 +36,7 @@ struct orbr_state {
     double* d_pose[2] = {};
     uint8_t* d_outl[2] = {};
     int* h_eoff = nullptr;   // pinned: edge_offset tables of both PoseOptimization calls ([2][n_frames + 1])
-    int h_eoff_cap = 0;
+    size_t h_eoff_bytes = 0;
     // chained flow: Frame::isInFrustum outputs per local map point + the frame's Sophus::SE3f after the first PoseOptimization
     int chain_np = -1;
     uint8_t* d_cview = nullptr;
@@ -170,21 +170,45 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     }
     const size_t rows_cap = h->out_rows;   // compact rows a batch of max_batch images can produce
     const bool po = S->pose_optimization != 0 || CH != nullptr;
-    // ---- carve the step's device block ----
+    cudaStream_t st = h->stream;
+    // ---- both eyes of every frame through the extractor, then ComputeStereoMatches; or the one image of every monocular frame
+    //      with vLappingArea = {0, 1000} (Frame.cc:380) and no stereo: mvuRight stays -1 for the searches and PoseOptimization ----
+    orb_status s = orbx_extract_batch(h, S->images, nimg, S->width, S->height, S->stride, S->image_stride_bytes, 0, mono ? 1000 : 0, nullptr, nullptr);
+    if (s != ORB_OK) return s;
+    if (!mono && (s = orbm_stereo_batch(h, nf, S->bf, S->b)) != ORB_OK) return s;
+    // ---- the step's device block, carved after the extraction is queued so that only the query copies precede the first search.
+    //      The chained flow and the local-map flow share the frame table, offsets, descriptors and world positions of their queries ----
     struct Ptrs {
         int *fimgL, *qoffL, *dirL, *octL; float *tcwL, *xwL, *angL; uint8_t *descL, *obsL;
         int *fimgC, *qoffC, *lvlC; float *pxC, *pyC, *pxrC, *vcC, *tdC, *xwC; uint8_t *descC, *claimC, *viewC;
         float* pose;
         float *nrmK, *mxK, *mnK, *RcwK, *tcwK, *OwK; int* lastqK; uint8_t* seenK;
     } D{};
+    const int* fimgC = CH ? QL->frame_image : QC ? QC->frame_image : nullptr;
+    const int* qoffC = CH ? CH->point_offset : QC ? QC->query_offset : nullptr;
+    const uint8_t* descC = CH ? CH->desc : QC ? QC->desc : nullptr;
+    const float* xwC = CH ? CH->world_pos : po ? S->local_world_pos : nullptr;
     auto layout = [&](Carve& c) {
-        D.fimgL = c.take<int>(nf); D.qoffL = c.take<int>(nf + 1); D.dirL = c.take<int>(nf); D.tcwL = c.take<float>((size_t)nf * 7);
-        D.xwL = c.take<float>((size_t)nqL * 3); D.octL = c.take<int>(nqL); D.angL = c.take<float>(nqL); D.descL = c.take<uint8_t>((size_t)nqL * 32);
-        D.obsL = c.take<uint8_t>(nqL);
-        D.fimgC = c.take<int>(nf); D.qoffC = c.take<int>(nf + 1); D.pxC = c.take<float>(nqC); D.pyC = c.take<float>(nqC); D.pxrC = c.take<float>(nqC);
-        D.lvlC = c.take<int>(nqC); D.vcC = c.take<float>(nqC); D.tdC = c.take<float>(nqC); D.descC = c.take<uint8_t>((size_t)nqC * 32);
-        D.claimC = c.take<uint8_t>(rows_cap); D.viewC = c.take<uint8_t>(nqC); D.xwC = c.take<float>((size_t)nqC * 3);
-        D.pose = c.take<float>((size_t)nf * 7);
+        if (QL) {
+            D.fimgL = stage_in(c, QL->frame_image, nf, false); D.qoffL = stage_in(c, QL->query_offset, nf + 1, false);
+            D.dirL = stage_in(c, QL->direction, nf, false); D.tcwL = stage_in(c, QL->Tcw, (size_t)nf * 7, false);
+            D.xwL = stage_in(c, QL->world_pos, (size_t)nqL * 3, false); D.octL = stage_in(c, QL->last_octave, nqL, false);
+            D.angL = stage_in(c, QL->last_angle, nqL, false); D.descL = stage_in(c, QL->desc, (size_t)nqL * 32, false);
+            D.obsL = stage_in(c, QL->obs_positive, nqL, false);
+        }
+        D.fimgC = stage_in(c, fimgC, nf, false); D.qoffC = stage_in(c, qoffC, nf + 1, false);
+        D.descC = stage_in(c, descC, (size_t)nqC * 32, false); D.xwC = stage_in(c, xwC, (size_t)nqC * 3, false);
+        if (QC) {
+            D.pxC = stage_in(c, QC->proj_x, nqC, false); D.pyC = stage_in(c, QC->proj_y, nqC, false); D.pxrC = stage_in(c, QC->proj_xr, nqC, false);
+            D.lvlC = stage_in(c, QC->level, nqC, false); D.vcC = stage_in(c, QC->view_cos, nqC, false); D.tdC = stage_in(c, QC->track_depth, nqC, false);
+            D.viewC = stage_in(c, QC->in_view, nqC, false);
+        }
+        if (CH) {
+            D.nrmK = stage_in(c, CH->normal, (size_t)nqC * 3, false); D.mxK = stage_in(c, CH->max_dist, nqC, false);
+            D.mnK = stage_in(c, CH->min_dist, nqC, false); D.lastqK = stage_in(c, CH->last_query, nqC, false);
+        }
+        D.pose = stage_in(c, po ? S->pose : nullptr, (size_t)nf * 7, false);
+        D.claimC = c.take<uint8_t>(rows_cap);
         r->d_fm = c.take<int>(rows_cap); r->d_nm_last = c.take<int>(nf); r->d_match = c.take<int>(nqC); r->d_nm_local = c.take<int>(nf);
         for (int k = 0; k < 2; ++k) {
             r->d_eoff[k] = c.take<int>(nf + 1); r->d_efeat[k] = c.take<int>(po ? rows_cap : 1); r->d_inl[k] = c.take<int>(nf);
@@ -192,44 +216,21 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         }
         r->d_exw = c.take<float>(po ? rows_cap * 3 : 1); r->d_eobs = c.take<float>(po ? rows_cap * 3 : 1); r->d_ew = c.take<float>(po ? rows_cap : 1);
         const size_t npK = CH ? (size_t)nqC : 0;
-        D.nrmK = c.take<float>(npK * 3); D.mxK = c.take<float>(npK); D.mnK = c.take<float>(npK); D.lastqK = c.take<int>(npK);
         D.RcwK = c.take<float>((size_t)nf * 9); D.tcwK = c.take<float>((size_t)nf * 3); D.OwK = c.take<float>((size_t)nf * 3);
         D.seenK = c.take<uint8_t>(CH ? (size_t)nqL : 0);
         r->d_cview = c.take<uint8_t>(npK); r->d_cpx = c.take<float>(npK); r->d_cpy = c.take<float>(npK); r->d_cpxr = c.take<float>(npK);
         r->d_clevel = c.take<int>(npK); r->d_cvc = c.take<float>(npK); r->d_cdepth = c.take<float>(npK); r->d_posef = c.take<float>((size_t)nf * 7);
     };
-    orb_status s = carve_scratch(r->bytes, r->d_buf, h->capturing, h->stream, layout).status;
-    if (s != ORB_OK) return s;
-    if (r->h_eoff_cap < 2 * (nf + 1)) {
-        if (r->h_eoff) cudaFreeHost(r->h_eoff);
-        r->h_eoff = nullptr;
-        ORB_CUDA(cudaMallocHost((void**)&r->h_eoff, sizeof(int) * 2 * (nf + 1)));
-        r->h_eoff_cap = 2 * (nf + 1);
-    }
-    cudaStream_t st = h->stream;
-    // ---- both eyes of every frame through the extractor, then ComputeStereoMatches; or the one image of every monocular frame
-    //      with vLappingArea = {0, 1000} (Frame.cc:380) and no stereo: mvuRight stays -1 for the searches and PoseOptimization ----
-    s = orbx_extract_batch(h, S->images, nimg, S->width, S->height, S->stride, S->image_stride_bytes, 0, mono ? 1000 : 0, nullptr, nullptr);
-    if (s != ORB_OK) return s;
-    if (!mono && (s = orbm_stereo_batch(h, nf, S->bf, S->b)) != ORB_OK) return s;
-    auto up = [&](void* dst, const void* src, size_t bytes) -> orb_status {
-        if (src && bytes) ORB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
-        return ORB_OK;
-    };
+    if ((s = carve_scratch(r->bytes, r->d_buf, h->capturing, st, layout).status) != ORB_OK ||
+        (s = grow_pinned(r->h_eoff_bytes, r->h_eoff, sizeof(int) * 2 * (nf + 1))) != ORB_OK)
+        return s;
     const int qb0 = h->q_total_bound, qb1 = h->q_frame_bound, qb2 = h->rows_bound;
     auto restore = [&]() { h->q_total_bound = qb0; h->q_frame_bound = qb1; h->rows_bound = qb2; };
-    if (po && (s = up(D.pose, S->pose, sizeof(float) * 7 * (size_t)nf)) != ORB_OK) return s;
     // ---- TrackWithMotionModel: SearchByProjection(cur, last) [+ PoseOptimization] ----
     if (QL) {
-        if ((s = up(D.fimgL, QL->frame_image, 4 * (size_t)nf)) != ORB_OK || (s = up(D.qoffL, QL->query_offset, 4 * (size_t)(nf + 1))) != ORB_OK ||
-            (s = up(D.tcwL, QL->Tcw, 28 * (size_t)nf)) != ORB_OK || (s = up(D.dirL, QL->direction, 4 * (size_t)nf)) != ORB_OK ||
-            (s = up(D.xwL, QL->world_pos, 12 * (size_t)nqL)) != ORB_OK || (s = up(D.octL, QL->last_octave, 4 * (size_t)nqL)) != ORB_OK ||
-            (s = up(D.angL, QL->last_angle, 4 * (size_t)nqL)) != ORB_OK || (s = up(D.descL, QL->desc, 32 * (size_t)nqL)) != ORB_OK ||
-            (s = up(D.obsL, QL->obs_positive, (size_t)nqL)) != ORB_OK)
-            return s;
         orbm_last_queries q{};
         q.n_frames = nf; q.on_device = 1; q.frame_image = D.fimgL; q.query_offset = D.qoffL; q.Tcw = D.tcwL; q.direction = D.dirL;
-        q.world_pos = D.xwL; q.last_octave = D.octL; q.last_angle = D.angL; q.desc = D.descL; q.obs_positive = QL->obs_positive ? D.obsL : nullptr;
+        q.world_pos = D.xwL; q.last_octave = D.octL; q.last_angle = D.angL; q.desc = D.descL; q.obs_positive = D.obsL;
         h->q_total_bound = std::max(nqL, 1); h->q_frame_bound = std::max(maxqL, 1); h->rows_bound = (int)rows_cap;   // exact: the host tables are at hand
         s = orbm_search_last_frame(h, cam, &q, S->th_last, S->check_orientation_last, r->d_fm, r->d_nm_last);
         restore();
@@ -244,14 +245,8 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     }
     // ---- the chained flow: outlier release, pose -> Sophus::SE3f, isInFrustum, local-map search, second PoseOptimization ----
     if (CH) {
-        const int np = nqC;
-        if ((s = up(D.fimgC, QL->frame_image, 4 * (size_t)nf)) != ORB_OK || (s = up(D.qoffC, CH->point_offset, 4 * (size_t)(nf + 1))) != ORB_OK ||
-            (s = up(D.xwC, CH->world_pos, 12 * (size_t)np)) != ORB_OK || (s = up(D.nrmK, CH->normal, 12 * (size_t)np)) != ORB_OK ||
-            (s = up(D.mxK, CH->max_dist, 4 * (size_t)np)) != ORB_OK || (s = up(D.mnK, CH->min_dist, 4 * (size_t)np)) != ORB_OK ||
-            (s = up(D.descC, CH->desc, 32 * (size_t)np)) != ORB_OK || (s = up(D.lastqK, CH->last_query, 4 * (size_t)np)) != ORB_OK)
-            return s;
         ORB_CUDA(cudaMemsetAsync(D.seenK, 0, std::max(nqL, 1), st));
-        k_chain_after_motion<<<nf, 256, 0, st>>>(D.fimgL, h->d_offsets, h->d_nkp, h->geom.kpTotal, D.qoffL, QL->obs_positive ? D.obsL : nullptr, r->d_eoff[0],
+        k_chain_after_motion<<<nf, 256, 0, st>>>(D.fimgL, h->d_offsets, h->d_nkp, h->geom.kpTotal, D.qoffL, D.obsL, r->d_eoff[0],
                                                  r->d_efeat[0], r->d_outl[0], r->d_pose[0], r->d_fm, D.seenK, D.claimC, r->d_posef, D.RcwK, D.tcwK, D.OwK);
         ORB_LAUNCHED();
         orbf_frustum_points fp{};
@@ -267,7 +262,7 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         orbm_local_queries q{};
         q.n_frames = nf; q.on_device = 1; q.frame_image = D.fimgC; q.query_offset = D.qoffC; q.proj_x = r->d_cpx; q.proj_y = r->d_cpy; q.proj_xr = r->d_cpxr;
         q.level = r->d_clevel; q.view_cos = r->d_cvc; q.track_depth = r->d_cdepth; q.desc = D.descC; q.feature_claimed = D.claimC; q.in_view = r->d_cview;
-        h->q_total_bound = std::max(np, 1); h->q_frame_bound = std::max(maxqC, 1); h->rows_bound = (int)rows_cap;
+        h->q_total_bound = std::max(nqC, 1); h->q_frame_bound = std::max(maxqC, 1); h->rows_bound = (int)rows_cap;
         s = orbm_search_local_points(h, cam, &q, S->th_local, S->nnratio_local, S->far_points, S->th_far, r->d_match, r->d_nm_local);
         restore();
         if (s != ORB_OK) return s;
@@ -281,23 +276,16 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     }
     // ---- TrackLocalMap: SearchByProjection(F, local map points) [+ PoseOptimization] ----
     if (QC) {
-        if ((s = up(D.fimgC, QC->frame_image, 4 * (size_t)nf)) != ORB_OK || (s = up(D.qoffC, QC->query_offset, 4 * (size_t)(nf + 1))) != ORB_OK ||
-            (s = up(D.pxC, QC->proj_x, 4 * (size_t)nqC)) != ORB_OK || (s = up(D.pyC, QC->proj_y, 4 * (size_t)nqC)) != ORB_OK ||
-            (s = up(D.pxrC, QC->proj_xr, 4 * (size_t)nqC)) != ORB_OK || (s = up(D.lvlC, QC->level, 4 * (size_t)nqC)) != ORB_OK ||
-            (s = up(D.vcC, QC->view_cos, 4 * (size_t)nqC)) != ORB_OK || (s = up(D.tdC, QC->track_depth, 4 * (size_t)nqC)) != ORB_OK ||
-            (s = up(D.descC, QC->desc, 32 * (size_t)nqC)) != ORB_OK || (s = up(D.viewC, QC->in_view, (size_t)nqC)) != ORB_OK)
-            return s;
         if (QC->feature_claimed) return set_error(ORB_ERR_UNSUPPORTED, "orbr_submit: feature_claimed refers to rows that do not exist yet; pass NULL");
         orbm_local_queries q{};
         q.n_frames = nf; q.on_device = 1; q.frame_image = D.fimgC; q.query_offset = D.qoffC; q.proj_x = D.pxC; q.proj_y = D.pyC; q.proj_xr = D.pxrC;
-        q.level = D.lvlC; q.view_cos = D.vcC; q.track_depth = QC->track_depth ? D.tdC : nullptr; q.desc = D.descC; q.feature_claimed = nullptr;
-        q.in_view = QC->in_view ? D.viewC : nullptr;
+        q.level = D.lvlC; q.view_cos = D.vcC; q.track_depth = D.tdC; q.desc = D.descC; q.feature_claimed = nullptr;
+        q.in_view = D.viewC;
         h->q_total_bound = std::max(nqC, 1); h->q_frame_bound = std::max(maxqC, 1); h->rows_bound = (int)rows_cap;
         s = orbm_search_local_points(h, cam, &q, S->th_local, S->nnratio_local, S->far_points, S->th_far, r->d_match, r->d_nm_local);
         restore();
         if (s != ORB_OK) return s;
         if (po) {
-            if ((s = up(D.xwC, S->local_world_pos, 12 * (size_t)nqC)) != ORB_OK) return s;
             orbo_edge_source es{nf, D.fimgC, nullptr, D.qoffC, r->d_match, D.xwC};
             if ((s = orbo_pose_edges(h, &es, r->d_eoff[1], r->d_efeat[1], r->d_exw, r->d_eobs, r->d_ew)) != ORB_OK) return s;
             orbo_pose_problems pp{nf, 1, r->d_eoff[1], D.pose, r->d_exw, r->d_eobs, r->d_ew, cam->fx, cam->fy, cam->cx, cam->cy, cam->bf, (int32_t)rows_cap};
@@ -306,9 +294,7 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         }
     }
     // ---- the small tables back: per-image counts / offsets and the capacity flags ----
-    const int MB = h->cfg.max_batch;
-    ORB_CUDA(cudaMemcpyAsync(h->h_counts, h->d_nkp, sizeof(int) * (3 * MB + 1), cudaMemcpyDeviceToHost, st));
-    ORB_CUDA(cudaMemcpyAsync(h->h_counts + 3 * MB + 4, h->d_err, sizeof(int) * 4, cudaMemcpyDeviceToHost, st));
+    if ((s = queue_counts(h)) != ORB_OK) return s;
     ORB_CUDA(cudaEventRecord(r->ev_counts, st));
     r->pending = true;
     r->n_frames = nf; r->nimg = nimg; r->mono = mono;
@@ -322,25 +308,19 @@ extern "C" orb_status orbr_collect(orbx_handle* h, const orbr_results* O, int32_
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     ORB_CUDA(cudaEventSynchronize(r->ev_counts));
     r->pending = false;
-    const int MB = h->cfg.max_batch, nimg = r->nimg, nf = r->n_frames;
-    h->counts_valid = true;
-    const int* e = h->h_counts + 3 * MB + 4;
-    h->batch_status = (e[0] || e[1]) ? (e[0] ? 1 : 2) : 0;
-    if (h->batch_status) {
-        cudaMemsetAsync(h->d_err, 0, sizeof(int) * 8, h->stream);
-        return set_error(ORB_ERR_CAPACITY, h->batch_status == 1 ? "FAST candidate capacity exceeded" : "quadtree node capacity exceeded");
-    }
-    const int rows = h->h_counts[2 * MB + nimg];
+    const int nimg = r->nimg, nf = r->n_frames;
+    orb_status s = latch_counts(h);
+    if (s != ORB_OK) return s;
+    const int rows = image_row0(h, nimg);
     if (total_rows_out) *total_rows_out = rows;
-    if (O->n) for (int b = 0; b < nimg; ++b) O->n[b] = h->h_counts[b];
-    if (O->offsets) for (int b = 0; b <= nimg; ++b) O->offsets[b] = h->h_counts[2 * MB + b];
+    if (O->n) for (int b = 0; b < nimg; ++b) O->n[b] = image_features(h, b);
+    if (O->offsets) for (int b = 0; b <= nimg; ++b) O->offsets[b] = image_row0(h, b);
     if (rows > O->cap_rows) return set_error(ORB_ERR_CAPACITY, "result buffers smaller than the batch result");
     cudaStream_t st = h->stream;
     auto down = [&](void* dst, const void* src, size_t bytes) -> orb_status {
         if (dst && bytes) ORB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st));
         return ORB_OK;
     };
-    orb_status s;
     if ((s = down(O->keypoints, h->d_kps, sizeof(orbx_keypoint) * (size_t)rows)) != ORB_OK || (s = down(O->descriptors, h->d_desc, 32 * (size_t)rows)) != ORB_OK)
         return s;
     if (r->mono) {   // the monocular Frame stores mvuRight = mvDepth = -1; d_uright may still hold an earlier stereo batch

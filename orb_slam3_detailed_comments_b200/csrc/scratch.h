@@ -1,25 +1,29 @@
-// scratch.h -- per-call device scratch: one carver, one growth policy, one staging helper for each direction (host code only)
+// scratch.h -- device memory described once: one carver, one growth policy for per-call blocks, one exact-size block for
+// long-lived state, and one staging helper for each direction (host code only)
 //
-// An entry point describes its scratch block once, as a `layout` function of a Carve that assigns every device pointer.
-// carve_scratch runs it with a null base to measure, grows the buffer to fit and runs it again on the buffer, so the size
-// always matches what the layout takes.
+// A caller describes its block once, as a `layout` function of a Carve that assigns every device pointer.  The layout runs once with
+// a null base to measure and once on the block to fill, so the size always matches what the layout takes.  carve_scratch grows a
+// per-call buffer to fit (with headroom); carve_exact allocates a block of exactly the measured size, once.
 //
-// Arrays an entry point takes in or returns name the caller's pointer once in the layout.  stage_in gives a device caller its own
+// Arrays a caller takes in or returns name the caller's pointer once in the layout.  stage_in gives a device caller its own
 // pointer back and copies a host array into a slot of the block.  stage_out gives a device caller its own pointer back and gives a
 // host caller a slot whose contents copy_out later copies to the caller's array; an in-out array is staged in and then named in
 // a copy_back.  copy_out issues every recorded copy and waits for the stream, so a host-form call ends with it and a device-form
 // call, which records none, never calls it.
 //
-// Some calls nest, so a call never carves the arena its caller carves.  Which entry points use which buffer:
+// Some calls nest, so a call never carves the arena its caller carves.  Which blocks are carved where:
 //
-// | Buffer | Entry points |
-// |---|---|
-// | `h->d_stage` | every matcher.cu entry point, `orbm_search_triangulation`, `orbo_pose_optimization`, `orbo_pose_edges` (its count array) |
-// | `h->d_po` | `orbo_pose_optimization_frames` (it calls the two above), `orbv_transform`, `orbp_distinctive_descriptors`, `orbp_update_normal_and_depth`, `orbm_hamming_knn2` |
-// | `orbr_state::d_buf` | `orbr_submit` (it calls the searches and pose calls above) |
-// | `h->d_xl` | the frame blocks of the matcher searches' global-memory form (matcher.cu `launch_proj`) |
+// | Block | Carved by | Entry points |
+// |---|---|---|
+// | `h->d_ws` | carve_exact | `orbx_create`: the extractor handle's workspace for max_width x max_height x max_batch (extractor.cu) |
+// | `orbv_vocabulary::d_buf` | carve_exact | `orbv_create`: the vocabulary tree (bow.cu) |
+// | `h->d_stage` | carve_scratch | every matcher.cu entry point, `orbm_search_triangulation`, `orbo_pose_optimization`, `orbo_pose_edges` (its count array) |
+// | `h->d_po` | carve_scratch | `orbo_pose_optimization_frames` (it calls the two above), `orbv_transform`, `orbp_distinctive_descriptors`, `orbp_update_normal_and_depth`, `orbm_hamming_knn2` |
+// | `orbr_state::d_buf` | carve_scratch | `orbr_submit` (it calls the searches and pose calls above) |
+// | `h->d_xl` | grow_device | the frame blocks of the matcher searches' global-memory form (matcher.cu `launch_proj`) |
 //
-// Captured CUDA graphs hold pointers into these buffers, so a buffer only grows in an eager call: growth inside a capture is refused.
+// Captured CUDA graphs hold pointers into these buffers, so a per-call buffer only grows in an eager call: growth inside a capture is
+// refused.  The exact-size blocks never grow.
 //
 // The two bundle-adjustment solvers (`lba_solve*`, `liba_solve`) are not carved: each lays a batch out in its handle's `d_buf` with
 // a pinned mirror in `h_buf` (pack.h), both grown by the functions below.
@@ -108,7 +112,8 @@ inline orb_status grow_device(size_t& bytes, uint8_t*& ptr, size_t need, bool ca
     return ORB_OK;
 }
 
-inline orb_status grow_pinned(size_t& bytes, uint8_t*& ptr, size_t need) {
+template <typename T>
+orb_status grow_pinned(size_t& bytes, T*& ptr, size_t need) {
     if (need <= bytes) return ORB_OK;
     if (ptr) cudaFreeHost(ptr);
     ptr = nullptr;
@@ -171,6 +176,22 @@ Carve carve_scratch(size_t& bytes, uint8_t*& ptr, bool capturing, cudaStream_t s
     const orb_status s = grow_device(bytes, ptr, m.off, capturing);
     if (s != ORB_OK) {
         m.status = s;
+        return m;
+    }
+    Carve c{ptr, stream};
+    layout(c);
+    return c;
+}
+
+// measure `layout`, allocate exactly that many bytes into `ptr` (no headroom: the block is allocated once and kept) and carve it:
+// returns the filled carve, whose status is the first error of the allocation or of a stage_in copy
+template <typename F>
+Carve carve_exact(uint8_t*& ptr, cudaStream_t stream, F&& layout) {
+    Carve m{nullptr, stream};
+    layout(m);
+    if (cudaMalloc((void**)&ptr, m.off) != cudaSuccess) {
+        ptr = nullptr;
+        m.status = set_error(ORB_ERR_CUDA, "cudaMalloc of " + std::to_string(m.off) + " B failed");
         return m;
     }
     Carve c{ptr, stream};

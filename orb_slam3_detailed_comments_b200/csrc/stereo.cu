@@ -343,17 +343,22 @@ extern "C" orb_status orbm_stereo_batch(orbx_handle* h, int32_t n_pairs, float b
     return run_stereo(h, h, n_pairs, 2, 0, 2, 1, bf, b);
 }
 
-extern "C" orb_status orbm_stereo_download(orbx_handle* h, float* uright, float* depth, int32_t cap_rows) {
-    int total = 0;
-    orb_status s = batch_rows(h, &total);
-    if (s != ORB_OK) return s;
-    const int rows = std::min(total, (int)cap_rows);
+// the uright / depth rows [0, n) of the last stereo batch, as many as the caller's `cap` rows hold
+static orb_status download_stereo_rows(orbx_handle* h, int n, float* uright, float* depth, int32_t cap, const char* too_small) {
+    const int rows = std::min(n, (int)cap);
     if (rows > 0) {
         if (uright) ORB_CUDA(cudaMemcpyAsync(uright, h->d_uright, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));
         if (depth) ORB_CUDA(cudaMemcpyAsync(depth, h->d_depth, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));
         ORB_CUDA(cudaStreamSynchronize(h->stream));
     }
-    return total > cap_rows ? set_error(ORB_ERR_CAPACITY, "output buffer smaller than the batch result") : ORB_OK;
+    return n > cap ? set_error(ORB_ERR_CAPACITY, too_small) : ORB_OK;
+}
+
+extern "C" orb_status orbm_stereo_download(orbx_handle* h, float* uright, float* depth, int32_t cap_rows) {
+    int total = 0;
+    orb_status s = batch_rows(h, &total);
+    if (s != ORB_OK) return s;
+    return download_stereo_rows(h, total, uright, depth, cap_rows, "output buffer smaller than the batch result");
 }
 
 extern "C" orb_status orbm_stereo_pair(orbx_handle* left, orbx_handle* right, float bf, float b, float* uright, float* depth,
@@ -362,12 +367,5 @@ extern "C" orb_status orbm_stereo_pair(orbx_handle* left, orbx_handle* right, fl
     if (s != ORB_OK) return s;
     s = orbx_counts(left, nullptr, nullptr, nullptr);
     if (s != ORB_OK) return s;
-    const int n = left->h_counts[0];
-    const int rows = std::min(n, (int)cap);
-    if (rows > 0) {
-        ORB_CUDA(cudaMemcpyAsync(uright, left->d_uright, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, left->stream));
-        ORB_CUDA(cudaMemcpyAsync(depth, left->d_depth, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, left->stream));
-        ORB_CUDA(cudaStreamSynchronize(left->stream));
-    }
-    return n > cap ? set_error(ORB_ERR_CAPACITY, "output buffer smaller than N") : ORB_OK;
+    return download_stereo_rows(left, image_features(left, 0), uright, depth, cap, "output buffer smaller than N");
 }
