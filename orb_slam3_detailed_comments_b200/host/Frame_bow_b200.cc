@@ -7,7 +7,6 @@
 // DBoW2 fills them: BowVector entries in ascending word order, feature i under its node iff its word's weight is > 0
 // (TemplatedVocabulary.h:1153-1157).  The vocabulary's nodes are protected members of DBoW2::TemplatedVocabulary; they are read through
 // a derived class (no change to the reference's headers).  KeyFrame::ComputeBoW (KeyFrame.cc:101-112) has the same body.
-#include <cstdlib>
 #include <cstring>
 #include <map>
 #include <mutex>
@@ -16,7 +15,7 @@
 #include <vector>
 
 #include "Frame.h"             // the reference's header (here: the skeleton that stands in for it)
-#include "orb_b200_host.h"
+#include "marshal.h"
 
 namespace {
 
@@ -50,10 +49,8 @@ const orbv_vocabulary* device_vocabulary(const ORB_SLAM3::ORBVocabulary* voc) {
         if (i > 0 && !nd.descriptor.empty()) std::memcpy(&desc[(size_t)i * 32], nd.descriptor.template ptr<unsigned char>(), 32);   // the root has no descriptor
         if (nd.isLeaf() && i > 0) { word[i] = (int32_t)nd.word_id; weight[i] = nd.weight; }
     }
-    int dev = 0;
-    if (const char* d = std::getenv("ORB_B200_DEVICE")) dev = std::atoi(d);
     orbv_vocabulary* out = nullptr;
-    orb_b200::check(orbv_create(dev, n, VocabularyAccess::depth_levels(*voc), child_offset.data(), child_ids.data(), desc.data(), word.data(), weight.data(), &out),
+    orb_b200::check(orbv_create(orb_b200::device_ordinal(), n, VocabularyAccess::depth_levels(*voc), child_offset.data(), child_ids.data(), desc.data(), word.data(), weight.data(), &out),
                     "orbv_create");
     cache.byObject[voc] = out;
     return out;
@@ -65,12 +62,7 @@ namespace ORB_SLAM3 {
 
 void Frame::ComputeBoW() {
     if (!mBowVec.empty()) return;
-    if (Nleft != -1) throw orb_b200::Error("Frame::ComputeBoW: Nleft != -1 (fisheye stereo rig) is not built on the GPU path");
-    orbx_handle* h = orb_b200_handle_of(mpORBextractorLeft);
-    if (!h) throw orb_b200::Error("Frame::ComputeBoW: the frame's extractor is not a GPU-path extractor");
-    int32_t n = 0;
-    orb_b200::check(orbx_counts(h, &n, nullptr, nullptr), "orbx_counts");
-    if (n != N) throw orb_b200::Error("Frame::ComputeBoW: the frame is not the one its extractor produced last");
+    orbx_handle* h = orb_b200::resident_frame(*this, "Frame::ComputeBoW");
     mFeatVec.clear();
     if (N == 0) return;
     const orbv_vocabulary* voc = device_vocabulary(mpORBvocabulary);

@@ -17,7 +17,6 @@
 // which the stereo and matcher units look up per call.
 #include <algorithm>
 #include <cassert>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <unordered_map>
@@ -91,11 +90,7 @@ static orbx_handle* handle_for_image(const void* extractor, int w, int h) {
 extern "C" lba_handle* orb_b200_lba_handle(void) {
     Registry& r = registry();
     std::lock_guard<std::mutex> lk(r.mu);
-    if (!r.lba) {
-        int dev = 0;
-        if (const char* d = std::getenv("ORB_B200_DEVICE")) dev = std::atoi(d);
-        orb_b200::check(lba_create(dev, &r.lba), "lba_create");
-    }
+    if (!r.lba) orb_b200::check(lba_create(orb_b200::device_ordinal(), &r.lba), "lba_create");
     return r.lba;
 }
 
@@ -113,8 +108,7 @@ ORBextractor::ORBextractor(int _nfeatures, float _scaleFactor, int _nlevels, int
     cfg.max_width = ORB_B200_MAX_WIDTH;
     cfg.max_height = ORB_B200_MAX_HEIGHT;
     cfg.max_batch = 1;
-    cfg.device = 0;
-    if (const char* d = std::getenv("ORB_B200_DEVICE")) cfg.device = std::atoi(d);
+    cfg.device = orb_b200::device_ordinal();
     orbx_handle* h = nullptr;
     orb_b200::check(orbx_create(&cfg, &h), "orbx_create");
     {

@@ -16,7 +16,7 @@
 #include <vector>
 
 #include "ORBmatcher.h"        // the reference's header
-#include "orb_b200_host.h"
+#include "marshal.h"
 
 namespace ORB_SLAM3 {
 
@@ -37,28 +37,10 @@ int ORBmatcher::DescriptorDistance(const cv::Mat& a, const cv::Mat& b) {
     return d;
 }
 
-namespace {
-orbm_camera camera_of(const Frame& F) {
-    orbm_camera c;
-    c.fx = Frame::fx; c.fy = Frame::fy; c.cx = Frame::cx; c.cy = Frame::cy; c.bf = F.mbf; c.b = F.mb;
-    c.min_x = Frame::mnMinX; c.max_x = Frame::mnMaxX; c.min_y = Frame::mnMinY; c.max_y = Frame::mnMaxY;
-    return c;
-}
-orbx_handle* device_frame(const Frame& F, const char* who) {
-    if (F.Nleft != -1) throw orb_b200::Error(std::string(who) + ": Nleft != -1 (fisheye stereo rig) is not built on the GPU path");
-    orbx_handle* h = orb_b200_handle_of(F.mpORBextractorLeft);
-    if (!h) throw orb_b200::Error(std::string(who) + ": the frame's extractor is not a GPU-path extractor");
-    int32_t n = 0;
-    orb_b200::check(orbx_counts(h, &n, nullptr, nullptr), "orbx_counts");
-    if (n != F.N) throw orb_b200::Error(std::string(who) + ": the frame is not the one its extractor produced last");
-    return h;
-}
-}  // namespace
-
 // ORBmatcher.cc:45-239
 int ORBmatcher::SearchByProjection(Frame& F, const std::vector<MapPoint*>& vpMapPoints, const float th, const bool bFarPoints,
                                    const float thFarPoints) {
-    orbx_handle* h = device_frame(F, "ORBmatcher::SearchByProjection(Frame&, vpMapPoints)");
+    orbx_handle* h = orb_b200::resident_frame(F, "ORBmatcher::SearchByProjection(Frame&, vpMapPoints)");
     const int nq = (int)vpMapPoints.size();
     if (nq == 0) return 0;
     std::vector<float> px(nq), py(nq), pxr(nq), vcos(nq), depth(nq);
@@ -82,7 +64,7 @@ int ORBmatcher::SearchByProjection(Frame& F, const std::vector<MapPoint*>& vpMap
     q.n_frames = 1; q.on_device = 0; q.frame_image = &frame_image; q.query_offset = query_offset;
     q.proj_x = px.data(); q.proj_y = py.data(); q.proj_xr = pxr.data(); q.level = level.data(); q.view_cos = vcos.data();
     q.track_depth = depth.data(); q.desc = desc.data(); q.feature_claimed = claimed.data(); q.in_view = in_view.data();
-    const orbm_camera cam = camera_of(F);
+    const orbm_camera cam = orb_b200::camera_of(F);
     std::vector<int32_t> match(nq, -1);
     int32_t nmatches = 0;
     orb_b200::check(orbm_search_local_points(h, &cam, &q, th, mfNNratio, bFarPoints ? 1 : 0, thFarPoints, match.data(), &nmatches),
@@ -94,7 +76,7 @@ int ORBmatcher::SearchByProjection(Frame& F, const std::vector<MapPoint*>& vpMap
 
 // ORBmatcher.cc:1950-2184
 int ORBmatcher::SearchByProjection(Frame& CurrentFrame, const Frame& LastFrame, const float th, const bool bMono) {
-    orbx_handle* h = device_frame(CurrentFrame, "ORBmatcher::SearchByProjection(CurrentFrame, LastFrame)");
+    orbx_handle* h = orb_b200::resident_frame(CurrentFrame, "ORBmatcher::SearchByProjection(CurrentFrame, LastFrame)");
     if (LastFrame.Nleft != -1) throw orb_b200::Error("SearchByProjection(CurrentFrame, LastFrame): Nleft != -1 is not built");
     // :1964-1971, in the caller's own Sophus / Eigen float arithmetic
     const Sophus::SE3f Tcw = CurrentFrame.GetPose();
@@ -123,13 +105,12 @@ int ORBmatcher::SearchByProjection(Frame& CurrentFrame, const Frame& LastFrame, 
         std::memcpy(&desc[(size_t)k * 32], d.ptr<unsigned char>(), 32);
         obs[k] = pMP->Observations() > 0 ? 1 : 0;
     }
-    const Eigen::Quaternionf qc = Tcw.unit_quaternion();
-    const float T7[7] = {qc.x(), qc.y(), qc.z(), qc.w(), Tcw.translation()(0), Tcw.translation()(1), Tcw.translation()(2)};
+    const std::array<float, 7> T7 = orb_b200::pose7(Tcw);
     const int32_t frame_image = 0, query_offset[2] = {0, nq}, direction = bForward ? 1 : (bBackward ? 2 : 0);
     orbm_last_queries q;
-    q.n_frames = 1; q.on_device = 0; q.frame_image = &frame_image; q.query_offset = query_offset; q.Tcw = T7; q.direction = &direction;
+    q.n_frames = 1; q.on_device = 0; q.frame_image = &frame_image; q.query_offset = query_offset; q.Tcw = T7.data(); q.direction = &direction;
     q.world_pos = pos.data(); q.last_octave = octave.data(); q.last_angle = angle.data(); q.desc = desc.data(); q.obs_positive = obs.data();
-    const orbm_camera cam = camera_of(CurrentFrame);
+    const orbm_camera cam = orb_b200::camera_of(CurrentFrame);
     std::vector<int32_t> fmatch(CurrentFrame.N > 0 ? CurrentFrame.N : 1, -1);
     int32_t nmatches = 0;
     orb_b200::check(orbm_search_last_frame(h, &cam, &q, th, mbCheckOrientation ? 1 : 0, fmatch.data(), &nmatches), "orbm_search_last_frame");

@@ -5,12 +5,11 @@
 // and therefore still on the device -- else F2's own arrays are uploaded.  On the host: vnMatches12 sized to F1, the search call, and the
 // refresh of vbPrevMatched from the matches (:880-884).  Windows around vbPrevMatched, the level-0 rule, ratio test, match stealing through
 // vnMatches21 / vMatchedDistance and the rotation histogram are orbm_search_initialization.
-#include <cstring>
 #include <string>
 #include <vector>
 
 #include "ORBmatcher.h"        // the reference's header
-#include "orb_b200_host.h"
+#include "marshal.h"
 
 namespace ORB_SLAM3 {
 
@@ -22,32 +21,21 @@ int ORBmatcher::SearchForInitialization(Frame& F1, Frame& F2, std::vector<cv::Po
     const int n1 = (int)F1.mvKeysUn.size(), n2 = (int)F2.mvKeysUn.size();
     vnMatches12 = std::vector<int>(n1, -1);
     if (n1 == 0 || n2 == 0) return 0;
-    auto flatten = [](const Frame& F, int n, std::vector<orbx_keypoint>& kp, std::vector<uint8_t>& desc) {
-        kp.resize(n); desc.resize((size_t)n * 32);
-        for (int i = 0; i < n; ++i) {
-            const cv::KeyPoint& k = F.mvKeysUn[i];
-            kp[i].x = k.pt.x; kp[i].y = k.pt.y; kp[i].size = k.size; kp[i].angle = k.angle; kp[i].response = k.response; kp[i].octave = k.octave; kp[i].class_id = k.class_id;
-            std::memcpy(&desc[(size_t)i * 32], F.mDescriptors.ptr<unsigned char>(i), 32);
-        }
-    };
-    std::vector<orbx_keypoint> kp1, kp2;
-    std::vector<uint8_t> desc1, desc2;
-    flatten(F1, n1, kp1, desc1);
+    const orb_b200::Features f1 = orb_b200::features_of(F1.mvKeysUn, F1.mDescriptors, n1);
     std::vector<float> prev((size_t)n1 * 2);
     for (int i = 0; i < n1; ++i) { prev[2 * i] = vbPrevMatched[i].x; prev[2 * i + 1] = vbPrevMatched[i].y; }
     orbm_init_queries q;
-    q.n1 = n1; q.kp1 = kp1.data(); q.desc1 = desc1.data(); q.prev_matched = prev.data();
+    q.n1 = n1; q.kp1 = f1.kp.data(); q.desc1 = f1.desc.data(); q.prev_matched = prev.data();
     int32_t resident = -1;
     orb_b200::check(orbx_counts(h, &resident, nullptr, nullptr), "orbx_counts");
+    orb_b200::Features f2;
     if (resident == F2.N && F2.N == n2) {      // F2 is what its extractor produced last: search it where it lies
         q.n2 = 0; q.kp2 = nullptr; q.desc2 = nullptr; q.target_image = 0;
     } else {
-        flatten(F2, n2, kp2, desc2);
-        q.n2 = n2; q.kp2 = kp2.data(); q.desc2 = desc2.data(); q.target_image = -1;
+        f2 = orb_b200::features_of(F2.mvKeysUn, F2.mDescriptors, n2);
+        q.n2 = n2; q.kp2 = f2.kp.data(); q.desc2 = f2.desc.data(); q.target_image = -1;
     }
-    orbm_camera cam;
-    cam.fx = Frame::fx; cam.fy = Frame::fy; cam.cx = Frame::cx; cam.cy = Frame::cy; cam.bf = F2.mbf; cam.b = F2.mb;
-    cam.min_x = Frame::mnMinX; cam.max_x = Frame::mnMaxX; cam.min_y = Frame::mnMinY; cam.max_y = Frame::mnMaxY;
+    const orbm_camera cam = orb_b200::camera_of(F2);
     int32_t nmatches = 0;
     orb_b200::check(orbm_search_initialization(h, &cam, &q, windowSize, mfNNratio, mbCheckOrientation ? 1 : 0, vnMatches12.data(), &nmatches),
                     "orbm_search_initialization");

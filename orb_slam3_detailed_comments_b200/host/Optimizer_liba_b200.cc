@@ -19,7 +19,6 @@
 //  * `assert(mit->second >= 3)` (:2664) is compiled out of the reference's Release build; it is not evaluated here.
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <list>
 #include <map>
@@ -41,11 +40,7 @@ struct LibaRegistry {
 liba_handle* liba_handle_of_process() {   // one LocalInertialBA workspace per process (created on first use, released at exit)
     static LibaRegistry r;
     std::lock_guard<std::mutex> lk(r.mu);
-    if (!r.h) {
-        int dev = 0;
-        if (const char* d = std::getenv("ORB_B200_DEVICE")) dev = std::atoi(d);
-        orb_b200::check(liba_create(dev, &r.h), "liba_create");
-    }
+    if (!r.h) orb_b200::check(liba_create(orb_b200::device_ordinal(), &r.h), "liba_create");
     return r.h;
 }
 

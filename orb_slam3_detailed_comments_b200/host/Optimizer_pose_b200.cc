@@ -11,7 +11,7 @@
 #include <vector>
 
 #include "Optimizer.h"        // the reference's header
-#include "orb_b200_host.h"
+#include "marshal.h"
 
 namespace ORB_SLAM3 {
 
@@ -42,11 +42,10 @@ int Optimizer::PoseOptimization(Frame* pFrame) {
     if (nInitialCorrespondences < 3) return 0;   // :292-293
 
     const Sophus::SE3<float> Tcw = pFrame->GetPose();
-    const float pose[7] = {Tcw.unit_quaternion().x(), Tcw.unit_quaternion().y(), Tcw.unit_quaternion().z(), Tcw.unit_quaternion().w(),
-                           Tcw.translation()(0), Tcw.translation()(1), Tcw.translation()(2)};
+    const std::array<float, 7> pose = orb_b200::pose7(Tcw);
     const int32_t edge_offset[2] = {0, nInitialCorrespondences};
     orbo_pose_problems in;
-    in.n_frames = 1; in.on_device = 0; in.edge_offset = edge_offset; in.pose = pose;
+    in.n_frames = 1; in.on_device = 0; in.edge_offset = edge_offset; in.pose = pose.data();
     in.world_pos = world_pos.data(); in.obs = obs.data(); in.inv_sigma2 = inv_sigma2.data();
     in.fx = pFrame->fx; in.fy = pFrame->fy; in.cx = pFrame->cx; in.cy = pFrame->cy; in.bf = pFrame->mbf;
     in.n_edges_max = nInitialCorrespondences;

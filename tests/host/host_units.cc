@@ -24,7 +24,6 @@
 #include "orb_b200_host.h"
 
 using namespace ORB_SLAM3;
-extern "C" void orb_b200_use_handle_for_keyframe_searches(orbx_handle* h);   // host/ORBmatcher_bow_b200.cc
 
 static std::string g_dir;
 template <typename T>

@@ -2,8 +2,9 @@
 include/ORBextractor.h, include/ORBmatcher.h, include/Optimizer.h, unchanged -- and define exactly the members they replace.
 Frame / KeyFrame / MapPoint / Map come from host/refshim/ref_skeleton.h (their real headers pull in Sophus, g2o, DBoW2, boost and
 Pangolin, none of which exist here); every skeleton member is checked, line by line, against the text of the reference header it
-claims to restate.  Needs /root/reference, so it only runs in the build container; tests/test_zz_host_boundary_gpu.py RUNS the
-same translation units on an H100."""
+claims to restate.  Without a reference checkout the units compile against the stand-in declarations of tests/host/refdecl instead,
+with the same defines and symbol checks; only the line-by-line check of the skeleton needs the checkout.
+tests/test_zz_host_boundary_gpu.py and tests/test_zz_host_units_gpu.py RUN the same translation units on an H100."""
 import os
 import re
 import subprocess
@@ -15,14 +16,16 @@ from oracle.pyoracle import REFERENCE_ROOT
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF = REFERENCE_ROOT
 HOST = os.path.join(ROOT, "orb_slam3_detailed_comments_b200", "host")
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "include", "ORBmatcher.h")), reason="reference checkout not present")
+HAVE_REF = os.path.exists(os.path.join(REF, "include", "ORBmatcher.h"))
+# the reference's own class declarations when a checkout is present, else the stand-ins (as tests/host/build.sh chooses)
+DECL = ["-I", os.path.join(REF, "include"), "-I", REF] if HAVE_REF else ["-I", os.path.join(ROOT, "tests", "host", "refdecl")]
 
 
 def _compile(tmp_path, name, *defines):
     obj = str(tmp_path / (name + ".o"))
     subprocess.check_call(["g++", "-std=c++14", "-Wall", "-Wno-comment", *defines, "-c", os.path.join(HOST, name + ".cc"),
                            "-include", os.path.join(HOST, "refshim", "ref_skeleton.h"), "-I", os.path.join(HOST, "refshim"),
-                           "-I", os.path.join(REF, "include"), "-I", REF, "-I", os.path.join(ROOT, "include"), "-I", HOST, "-o", obj])
+                           *DECL, "-I", os.path.join(ROOT, "include"), "-I", HOST, "-o", obj])
     return subprocess.check_output(["nm", "-C", obj], text=True)
 
 
@@ -83,10 +86,12 @@ def test_initialization_search_unit(tmp_path):
 
 
 def test_compute_bow_unit_and_its_vocabulary_access(tmp_path):
-    """Frame_bow_b200.cc against the skeleton (with a mock vocabulary whose nodes are protected, as in DBoW2), and the same access pattern
-    against the reference's REAL DBoW2 headers (over the boost / OpenCV miniatures of oracle/ref_shim)."""
+    """Frame_bow_b200.cc against the skeleton (with a mock vocabulary whose nodes are protected, as in DBoW2), and, with a reference
+    checkout, the same access pattern against the reference's REAL DBoW2 headers (over the boost / OpenCV miniatures of oracle/ref_shim)."""
     syms = _compile(tmp_path, "Frame_bow_b200", "-DORB_REFSHIM_VOC")
     assert "T ORB_SLAM3::Frame::ComputeBoW()" in syms and "U orbv_transform" in syms and "U orbv_create" in syms and "abort" not in syms
+    if not HAVE_REF:
+        return
     dbow = os.path.join(REF, "Thirdparty", "DBoW2")
     shim = os.path.join(ROOT, "oracle", "ref_shim")
     subprocess.check_call(["g++", "-std=c++14", "-Wall", "-Wno-comment", "-Wno-sign-compare", "-Wno-unused-variable", "-c", os.path.join(ROOT, "tests", "host", "voc_access_probe.cc"),
@@ -123,6 +128,7 @@ def _norm(s):
     return re.sub(r"\s+", "", re.sub(r"//.*", "", s))
 
 
+@pytest.mark.skipif(not HAVE_REF, reason="reference checkout not present")
 def test_skeleton_members_are_the_reference_declarations():
     """Every line between //@ref <header> and //@end in ref_skeleton.h appears verbatim (whitespace and comments aside) in that header."""
     text = open(os.path.join(HOST, "refshim", "ref_skeleton.h")).read().splitlines()
