@@ -89,6 +89,29 @@ orb_status orbx_extract_batch_device(orbx_handle* h, const uint8_t* d_imgs, int3
                                      int32_t height, int32_t stride, size_t image_stride_bytes,
                                      int32_t lap0, int32_t lap1);
 
+/* Pixel layout of a camera image: 8-bit channels, interleaved.  The colour formats are converted to grey as
+ * Tracking::GrabImageStereo / GrabImageMonocular do (Tracking.cc:1523-1601: cv::cvtColor with COLOR_RGB2GRAY / COLOR_BGR2GRAY
+ * for 3 channels, COLOR_RGBA2GRAY / COLOR_BGRA2GRAY for 4, chosen by mbRGB); alpha is ignored. */
+typedef enum {
+    ORB_FORMAT_GRAY = 0,
+    ORB_FORMAT_RGB = 1,
+    ORB_FORMAT_BGR = 2,
+    ORB_FORMAT_RGBA = 3,
+    ORB_FORMAT_BGRA = 4
+} orb_image_format;
+
+/* orbx_extract_batch_device for camera images of any orb_image_format and size: d_imgs holds `batch` images of
+ * src_width x src_height pixels in `format`, rows `stride` bytes apart, images image_stride_bytes apart (device memory).  Each is
+ * resized to width x height first when the sizes differ (System::TrackStereo / TrackMonocular's cv::resize(INTER_LINEAR) to
+ * Settings::newImSize, System.cc:286-298), channel by channel, then converted to grey, in the reference's order; the result is
+ * level 0 of the image's pyramid.  Keypoints are in the coordinates of the width x height image.  width / height are bounded by the
+ * handle's max_width / max_height, the source by nothing but memory.  src_width = src_height = 0 means width x height (no resize).
+ * Queues everything on the handle's stream with no synchronisation (graph capture works once the size has run eagerly); refuses an
+ * unknown format, a stride below src_width x channels or a size the handle cannot hold with ORB_ERR_INVALID before queuing. */
+orb_status orbx_extract_batch_device_format(orbx_handle* h, const uint8_t* d_imgs, int32_t batch, int32_t width, int32_t height,
+                                            int32_t stride, size_t image_stride_bytes, int32_t lap0, int32_t lap1,
+                                            int32_t format, int32_t src_width, int32_t src_height);
+
 /* Counts of the last batch: n[b] keypoints, mono_index[b]; offsets[b] = first row of image b in the
  * compact result arrays (offsets has batch+1 entries).  Synchronises the handle's stream. */
 /* upper bound of the keypoints of one image (row stride of per-image outputs such as orbv_transform's BowVector) */
@@ -685,6 +708,14 @@ typedef struct {
     const orbr_chain* chain;             /* NULL, or the chained flow: needs `last` and `pose`, `local` must be NULL; PoseOptimization runs after both
                                             searches whatever pose_optimization says; local_* results are indexed by the chain's map points */
     int32_t monocular;                   /* != 0: n_frames images, one per frame (Frame's monocular constructor), instead of 2 * n_frames stereo eyes */
+    /* Camera images as they arrive (orbx_extract_batch_device_format): all five zero = grey images of width x height laid out by
+       stride / image_stride_bytes above.  Otherwise `images` holds src_width x src_height images in image_format, laid out by
+       src_stride / src_image_stride_bytes, resized to width x height (when the sizes differ) and converted to grey on the device;
+       stride / image_stride_bytes are not read. */
+    int32_t image_format;                /* orb_image_format */
+    int32_t src_width, src_height;       /* 0 = width x height */
+    int32_t src_stride;                  /* bytes between rows; 0 = src_width x channels */
+    size_t src_image_stride_bytes;       /* bytes between images; 0 = src_stride x src_height */
 } orbr_step;
 
 typedef struct {                         /* HOST result buffers; any pointer may be NULL (that result is not copied back) */

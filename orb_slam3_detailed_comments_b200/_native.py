@@ -14,6 +14,10 @@ _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("ORB_LIB_PATH") or os.path.join(_PKG, "lib", "liborbslam3_b200.so")   # ORB_LIB_PATH: an instrumented build (tools/qt_phases.py)
 SOURCES = ["extractor.cu", "stereo.cu", "matcher.cu", "triangulation.cu", "lba.cu", "poseopt.cu", "bow.cu", "mappoint.cu", "liba.cu", "knn.cu", "replay.cu"]
 
+# k_ingest (the camera-image stage) is a shared object of its own beside the library, which opens it on first use (extractor.cu)
+INGEST_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_ingest.so")
+INGEST_SOURCES = ["ingest.cu"]
+
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
@@ -21,22 +25,29 @@ KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4
                      ("response", "<f4"), ("octave", "<i4"), ("class_id", "<i4")])
 
 
+# orb_image_format of include/orbslam3_b200.h, and the channels of each
+IMAGE_FORMATS = {"gray": 0, "rgb": 1, "bgr": 2, "rgba": 3, "bgra": 4}
+FORMAT_CHANNELS = {0: 1, 1: 3, 2: 3, 3: 4, 4: 4}
+
+
 class OrbError(RuntimeError):
     pass
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so (nvcc cross-compiles on CPU)."""
+    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so and lib/liborbslam3_b200_ingest.so (nvcc cross-compiles
+    on CPU)."""
     deps = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)] + [os.path.join(_PKG, "..", "include", "orbslam3_b200.h"),
                                                                    os.path.abspath(__file__)]   # the recipe itself
     if os.environ.get("ORB_LIB_PATH"):
         return LIB_PATH                       # an explicitly chosen build is never rebuilt
-    if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
-        return LIB_PATH
+    newest = max(os.path.getmtime(d) for d in deps)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     os.makedirs(os.path.dirname(LIB_PATH), exist_ok=True)
-    subprocess.check_call([nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB_PATH] +
-                          [os.path.join(_CSRC, s) for s in SOURCES])
+    for out, srcs in ((INGEST_LIB_PATH, INGEST_SOURCES), (LIB_PATH, SOURCES)):
+        if force or not os.path.exists(out) or os.path.getmtime(out) < newest:
+            subprocess.check_call([nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", out] +
+                                  [os.path.join(_CSRC, s) for s in srcs])
     return LIB_PATH
 
 
@@ -97,7 +108,8 @@ class orbr_step(C.Structure):
                 ("th_last", C.c_float), ("check_orientation_last", C.c_int32), ("local", C.POINTER(orbm_local_queries)),
                 ("th_local", C.c_float), ("nnratio_local", C.c_float), ("far_points", C.c_int32), ("th_far", C.c_float),
                 ("pose_optimization", C.c_int32), ("pose", C.c_void_p), ("local_world_pos", C.c_void_p), ("chain", C.POINTER(orbr_chain)),
-                ("monocular", C.c_int32)]
+                ("monocular", C.c_int32), ("image_format", C.c_int32), ("src_width", C.c_int32), ("src_height", C.c_int32),
+                ("src_stride", C.c_int32), ("src_image_stride_bytes", C.c_size_t)]
 
 
 class orbr_results(C.Structure):
@@ -174,6 +186,7 @@ SIGNATURES = {
     "orbx_extract": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP, _VP, _I, _IP, _IP]),
     "orbx_extract_batch": (_I, [_VP, _VP, _I, _I, _I, _I, C.c_size_t, _I, _I, _VP, _VP]),
     "orbx_extract_batch_device": (_I, [_VP, _VP, _I, _I, _I, _I, C.c_size_t, _I, _I]),
+    "orbx_extract_batch_device_format": (_I, [_VP, _VP, _I, _I, _I, _I, C.c_size_t, _I, _I, _I, _I, _I]),
     "orbx_counts": (_I, [_VP, _VP, _VP, _VP]),
     "orbx_download": (_I, [_VP, _VP, _VP, _I]),
     "orbx_level_size": (_I, [_VP, _I, _IP, _IP]),

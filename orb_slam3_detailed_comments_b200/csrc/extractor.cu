@@ -1,6 +1,7 @@
 // extractor.cu -- host side of the batched ORB extractor + its C ABI (include/orbslam3_b200.h).
 // Replaces ORBextractor::ORBextractor / operator() / ComputePyramid / ComputeKeyPointsOctTree
 // (/root/reference/src/ORBextractor.cc:468-571, 1557-1682, 1687-1738, 1061-1208).
+#include <dlfcn.h>
 #include <math.h>
 #include <string.h>
 
@@ -424,7 +425,7 @@ extern "C" void orbx_destroy(orbx_handle* h) {
     cudaSetDevice(h->cfg.device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     orbr_release(h);
-    for (void* p : {h->d_ws, h->d_stage, h->d_po, h->d_xl})
+    for (void* p : {h->d_ws, h->d_stage, h->d_po, h->d_xl, h->d_src})
         if (p) cudaFree(p);
     if (h->h_counts) cudaFreeHost(h->h_counts);
     for (int r = 0; r < orbx_handle::kProfRing; ++r)
@@ -592,6 +593,87 @@ extern "C" orb_status orbx_extract_batch_device(orbx_handle* h, const uint8_t* d
                                        stride, w, hh, cudaMemcpyDeviceToDevice, h->stream));
     }
     return run_pipeline(h, batch, lap0, lap1);
+}
+
+// ---- camera images of any format and size (k_ingest) ----------------------------------------------------------------------------
+static int format_channels(int format) { return format == ORB_FORMAT_GRAY ? 1 : format <= ORB_FORMAT_BGR ? 3 : 4; }
+
+// k_ingest lives in liborbslam3_b200_ingest.so next to this library (csrc/ingest.cu): its launcher, opened once on first use
+typedef cudaError_t (*IngestLaunch)(const orbdev::IngestPlan*, int32_t, int32_t, cudaStream_t);
+static orb_status ingest_launcher(IngestLaunch* out) {
+    static std::string err;
+    static const IngestLaunch fn = []() -> IngestLaunch {
+        Dl_info info;
+        if (!dladdr(reinterpret_cast<void*>(&orbx_create), &info) || !info.dli_fname) {
+            err = "dladdr failed";
+            return nullptr;
+        }
+        const std::string self(info.dli_fname), path = self.substr(0, self.rfind('/') + 1) + "liborbslam3_b200_ingest.so";
+        void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+        void* f = so ? dlsym(so, "orb_ingest_launch") : nullptr;
+        if (!f) {
+            const char* d = dlerror();
+            err = d ? d : path;
+        }
+        return reinterpret_cast<IngestLaunch>(f);
+    }();
+    *out = fn;
+    return fn ? ORB_OK : set_error(ORB_ERR_UNSUPPORTED, "the camera-image stage is missing (liborbslam3_b200_ingest.so next to the library): " + err);
+}
+
+orb_status check_source(ImageSource& src, int w, int hh) {
+    if (src.format < ORB_FORMAT_GRAY || src.format > ORB_FORMAT_BGRA) return set_error(ORB_ERR_INVALID, "unknown image format");
+    if (src.w == 0 && src.h == 0) { src.w = w; src.h = hh; }
+    const int64_t row = (int64_t)src.w * format_channels(src.format);
+    if (src.stride == 0) src.stride = row;
+    if (src.image_stride == 0) src.image_stride = (size_t)src.stride * src.h;
+    if (src.w < 1 || src.h < 1 || src.stride < row || src.stride > INT32_MAX) return set_error(ORB_ERR_INVALID, "bad source size or stride");
+    return ORB_OK;
+}
+
+extern "C" orb_status orbx_extract_batch_device_format(orbx_handle* h, const uint8_t* d_imgs, int32_t batch, int32_t w, int32_t hh,
+                                                       int32_t stride, size_t image_stride_bytes, int32_t lap0, int32_t lap1,
+                                                       int32_t format, int32_t src_width, int32_t src_height) {
+    ImageSource src{format, src_width, src_height, stride, image_stride_bytes};
+    if (!h) return set_error(ORB_ERR_INVALID, "null handle");
+    IngestLaunch launch = nullptr;
+    orb_status s = check_source(src, w, hh);
+    if (s == ORB_OK) s = ingest_launcher(&launch);
+    if (s == ORB_OK) s = check_batch_args(h, d_imgs, batch, w, hh, w);
+    if (s != ORB_OK) return s;
+    LevelGeom& L0 = h->geom.lv[0];
+    L0.base = h->d_pyr;
+    L0.pitch = round_up(w, 16);
+    L0.img_stride = (int64_t)L0.pitch * hh;
+    if (h->profiling) {
+        h->ev = h->evr[h->prof_count % orbx_handle::kProfRing];
+        ++h->prof_count;
+        cudaEventRecord(h->ev[0], h->stream);
+    }
+    const orbdev::IngestPlan P = orbdev::ig_plan(d_imgs, (int64_t)src.image_stride, format, src.w, src.h, (int)src.stride, L0.base, L0.img_stride,
+                                                 w, hh, L0.pitch);
+    const cudaError_t e = launch(&P, batch, h->cfg.device, h->stream);
+    if (e != cudaSuccess) return set_error(ORB_ERR_CUDA, std::string("k_ingest: ") + cudaGetErrorString(e));
+    ORB_LAUNCHED();
+    return run_pipeline(h, batch, lap0, lap1);
+}
+
+orb_status extract_batch_source(orbx_handle* h, const uint8_t* imgs, int batch, int w, int hh, const ImageSource& src, int lap0, int lap1) {
+    if (!imgs || batch < 1 || batch > h->cfg.max_batch) return set_error(ORB_ERR_INVALID, "bad batch");
+    if (w < 1 || hh < 1 || w > h->cfg.max_width || hh > h->cfg.max_height)
+        return set_error(ORB_ERR_INVALID, "image larger than the handle's max_width/max_height");
+    IngestLaunch launch = nullptr;
+    if (ingest_launcher(&launch) != ORB_OK) return ORB_ERR_UNSUPPORTED;   // before the upload
+    const size_t row = (size_t)src.w * format_channels(src.format), img = row * src.h;
+    ORB_CUDA(cudaSetDevice(h->cfg.device));
+    orb_status s = grow_device(h->src_bytes, h->d_src, img * batch, h->capturing);
+    if (s != ORB_OK) return s;
+    if (src.image_stride == (size_t)src.stride * src.h)   // the whole batch is one pitched 2-D copy
+        ORB_CUDA(cudaMemcpy2DAsync(h->d_src, row, imgs, src.stride, row, (size_t)src.h * batch, cudaMemcpyHostToDevice, h->stream));
+    else
+        for (int b = 0; b < batch; ++b)
+            ORB_CUDA(cudaMemcpy2DAsync(h->d_src + b * img, row, imgs + b * src.image_stride, src.stride, row, src.h, cudaMemcpyHostToDevice, h->stream));
+    return orbx_extract_batch_device_format(h, h->d_src, batch, w, hh, (int)row, img, lap0, lap1, src.format, src.w, src.h);
 }
 
 extern "C" orb_status orbx_extract_batch(orbx_handle* h, const uint8_t* imgs, int32_t batch, int32_t w, int32_t hh,

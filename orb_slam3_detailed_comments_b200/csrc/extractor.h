@@ -12,6 +12,14 @@ orb_status batch_rows(struct orbx_handle* h, int* rows);   // extractor.cu: comp
 orb_status queue_counts(struct orbx_handle* h);
 orb_status latch_counts(struct orbx_handle* h);
 
+// Camera images as they arrive (orbx_extract_batch_device_format, orbr_step): orb_image_format, size, row and image strides in bytes
+struct ImageSource { int format, w, h; int64_t stride; size_t image_stride; };
+// extractor.cu: fills the zero defaults of `src` (the size of the extracted w x hh image, tight strides) and refuses, before anything is
+// queued, an unknown format or a stride below a row of pixels
+orb_status check_source(ImageSource& src, int w, int hh);
+// extractor.cu: a batch of checked HOST images uploaded into the handle's staging block, then orbx_extract_batch_device_format
+orb_status extract_batch_source(struct orbx_handle* h, const uint8_t* imgs, int batch, int w, int hh, const ImageSource& src, int lap0, int lap1);
+
 struct orbx_handle {
     orbx_config cfg{};
     orb::ExtractGeom geom{};
@@ -84,6 +92,8 @@ struct orbx_handle {
     orbr_state* replay = nullptr;   // orbr_submit / orbr_collect state (replay.cu)
     uint8_t* d_xl = nullptr;        // frame blocks of the matcher's global-memory form (matcher.cu launch_proj)
     size_t xl_bytes = 0;
+    uint8_t* d_src = nullptr;       // host camera images of extract_batch_source, uploaded for k_ingest
+    size_t src_bytes = 0;
     int smem_optin = 0;             // cudaDevAttrMaxSharedMemoryPerBlockOptin of the handle's device, read on first use
 };
 

@@ -8,6 +8,8 @@
 // the small count tables back.  A monocular step (orbr_step::monocular) extracts one image per frame with vLappingArea = {0, 1000}
 // (Frame.cc:380) and skips ComputeStereoMatches; everything after the extraction is shared.  orbr_submit returns as soon as
 // everything is queued; orbr_collect waits for the counts, reads back exactly the rows the batch produced and waits once more.
+// Colour or differently sized camera images (orbr_step::image_format, src_*) go up as they are and become grey level-0 images on the
+// device (k_ingest) before the extraction.
 // A host thread that keeps several handles in flight (submit k+1 .. k+H-1 before collect k) overlaps uploads, kernels and
 // downloads of different handles without more threads.
 #include <string.h>
@@ -142,6 +144,13 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         return set_error(ORB_ERR_INVALID, "the chained flow needs `last` (with world positions), `pose`, no `local`, and every array of orbr_chain");
     if (S->pose_optimization && (!S->pose || (QL && !QL->world_pos) || (QC && !S->local_world_pos)))
         return set_error(ORB_ERR_INVALID, "pose_optimization needs pose and the world positions of the queries");
+    // camera images as they arrive: converted to grey and resized on the device (orbx_extract_batch_device_format)
+    ImageSource src{S->image_format, S->src_width, S->src_height, S->src_stride, S->src_image_stride_bytes};
+    const bool ingest = src.format || src.w || src.h || src.stride || src.image_stride;
+    if (ingest) {
+        const orb_status s = check_source(src, S->width, S->height);
+        if (s != ORB_OK) return s;
+    }
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     if (!h->replay) {
         h->replay = new orbr_state();
@@ -173,7 +182,8 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     cudaStream_t st = h->stream;
     // ---- both eyes of every frame through the extractor, then ComputeStereoMatches; or the one image of every monocular frame
     //      with vLappingArea = {0, 1000} (Frame.cc:380) and no stereo: mvuRight stays -1 for the searches and PoseOptimization ----
-    orb_status s = orbx_extract_batch(h, S->images, nimg, S->width, S->height, S->stride, S->image_stride_bytes, 0, mono ? 1000 : 0, nullptr, nullptr);
+    orb_status s = ingest ? extract_batch_source(h, S->images, nimg, S->width, S->height, src, 0, mono ? 1000 : 0)
+                          : orbx_extract_batch(h, S->images, nimg, S->width, S->height, S->stride, S->image_stride_bytes, 0, mono ? 1000 : 0, nullptr, nullptr);
     if (s != ORB_OK) return s;
     if (!mono && (s = orbm_stereo_batch(h, nf, S->bf, S->b)) != ORB_OK) return s;
     // ---- the step's device block, carved after the extraction is queued so that only the query copies precede the first search.

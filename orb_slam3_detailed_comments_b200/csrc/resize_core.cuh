@@ -39,19 +39,33 @@ ORB_HD uint32_t rs_dp2a_lo(uint32_t a, uint32_t b, uint32_t c) {  // c + a.lo16 
 #endif
 }
 
-// cv::resize INTER_LINEAR tap table (SURVEY App. A.1): {source index, c0 | c1 << 16} per destination coordinate (host)
+// One destination coordinate of cv::resize INTER_LINEAR (SURVEY App. A.1): source index *s and c0 | c1 << 16, scale = ssize / dsize.
+// clamp is the column rule (HResizeLinear's xmin / xmax): a tap before the first or at the last source pixel takes that pixel alone.
+// Rows keep the unclamped fraction and clip the two source rows to the image when they are read (resizeGeneric_), so an upscale's first
+// and last rows blend the edge row with itself at 1 - f / f, which rounds differently from the clamped tap.  A downscale (every
+// pyramid level) reaches neither border: the two rules give the same table there.
+ORB_HD uint32_t rs_tap(int d, double scale, int ssize, bool clamp, int* s) {
+#if defined(__CUDA_ARCH__)   // the host's rounding, operation by operation (no contraction)
+    float f = __double2float_rn(__dadd_rn(__dmul_rn(d + 0.5, scale), -0.5));
+#else
+    float f = (float)((d + 0.5) * scale - 0.5);
+#endif
+    *s = (int)floorf(f);
+    f -= (float)*s;
+    if (clamp && *s < 0) { *s = 0; f = 0.f; }
+    if (clamp && *s >= ssize - 1) { *s = ssize - 1; f = 0.f; }
+#if defined(__CUDA_ARCH__)
+    const int c0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f)), c1 = __float2int_rn(__fmul_rn(f, 2048.f));
+#else
+    const int c0 = (int)lrintf((1.f - f) * 2048.f), c1 = (int)lrintf(f * 2048.f);
+#endif
+    return (uint32_t)(c0 & 0xffff) | ((uint32_t)c1 << 16);
+}
+
+// cv::resize INTER_LINEAR tap table of a downscale: {source index, c0 | c1 << 16} per destination coordinate (host)
 inline void rs_linear_taps(int ssize, int dsize, int* out2) {
     const double scale = (double)ssize / dsize;
-    for (int d = 0; d < dsize; ++d) {
-        float f = (float)((d + 0.5) * scale - 0.5);
-        int s = (int)floorf(f);
-        f -= (float)s;
-        if (s < 0) { s = 0; f = 0.f; }
-        if (s >= ssize - 1) { s = ssize - 1; f = 0.f; }
-        const int c0 = (int)lrintf((1.f - f) * 2048.f), c1 = (int)lrintf(f * 2048.f);
-        out2[2 * d] = s;
-        out2[2 * d + 1] = (c0 & 0xffff) | (c1 << 16);
-    }
+    for (int d = 0; d < dsize; ++d) out2[2 * d + 1] = (int)rs_tap(d, scale, ssize, true, &out2[2 * d]);
 }
 
 struct RsTaps {          // the x taps of the thread's 4 destination pixels
@@ -129,6 +143,63 @@ ORB_HD void rs_thread(const uint8_t* src, int sw, int sh, int spitch, const uint
         if (dx4 + 4 > dw) packed &= 0xffffffffu >> (8 * (dx4 + 4 - dw));   // as k_resize: zero past the width
         *reinterpret_cast<uint32_t*>(dst + (int64_t)(dy0 + k) * dpitch + dx4) = packed;
     }
+}
+
+// ---- k_ingest: a camera image into level 0 -------------------------------------------------------------------------------
+// System::Track*'s cv::resize(INTER_LINEAR) of every channel of an interleaved u8 image, then Tracking::GrabImage*'s
+// cv::cvtColor(COLOR_{RGB,BGR}[A]2GRAY): gray = (k0 c0 + k1 c1 + k2 c2 + 2^14) >> 15 over the first three channels (alpha is
+// ignored) with OpenCV's 15-bit weights R 9798, G 19235, B 3735 in the image's channel order; a grey image has k = {32768, 0, 0}.
+struct IngestPlan {
+    const uint8_t* src;       // image 0
+    int64_t src_image;        // bytes between images
+    int sw, sh, spitch, cn;   // source size, row pitch in bytes, channels (1, 3, 4)
+    uint8_t* dst;             // level 0 of image 0
+    int64_t dst_image;
+    int dw, dh, dpitch;
+    int k[3];                 // grey weights of channels 0..2
+    int resize;               // source and destination sizes differ
+    double scale_x, scale_y;  // sw / dw, sh / dh
+};
+
+// the plan of a batch (host): format is an orb_image_format
+inline IngestPlan ig_plan(const uint8_t* src, int64_t src_image, int format, int sw, int sh, int spitch, uint8_t* dst, int64_t dst_image, int dw,
+                          int dh, int dpitch) {
+    static const int kWeights[5][3] = {{32768, 0, 0}, {9798, 19235, 3735}, {3735, 19235, 9798}, {9798, 19235, 3735}, {3735, 19235, 9798}};
+    const int cn = format == 0 ? 1 : format <= 2 ? 3 : 4;
+    return IngestPlan{src, src_image, sw, sh, spitch, cn, dst, dst_image, dw, dh, dpitch, {kWeights[format][0], kWeights[format][1], kWeights[format][2]},
+                      sw != dw || sh != dh, (double)sw / dw, (double)sh / dh};
+}
+
+// destination pixels dx4 .. dx4 + 3 of row dy of one image, packed; zero past the width
+ORB_HD uint32_t ig_pixels4(const IngestPlan& P, const uint8_t* src, int dx4, int dy) {
+    const int nc = P.cn < 3 ? P.cn : 3;
+    const uint8_t *r0 = src + (int64_t)dy * P.spitch, *r1 = r0;
+    int b0 = 0, b1 = 0;
+    if (P.resize) {
+        int sy;
+        const uint32_t cy = rs_tap(dy, P.scale_y, P.sh, false, &sy);
+        b0 = (int)(cy & 0xffffu); b1 = (int)(cy >> 16);
+        r0 = src + (int64_t)(sy < 0 ? 0 : sy) * P.spitch;
+        r1 = src + (int64_t)(sy + 1 < P.sh ? sy + 1 : P.sh - 1) * P.spitch;
+    }
+    uint32_t packed = 0;
+    for (int i = 0; i < 4 && dx4 + i < P.dw; ++i) {
+        int v[3] = {0, 0, 0};
+        if (P.resize) {
+            int x0;
+            const uint32_t cx = rs_tap(dx4 + i, P.scale_x, P.sw, true, &x0);
+            const int c0 = (int)(cx & 0xffffu), c1 = (int)(cx >> 16);
+            const int o0 = x0 * P.cn, o1 = (x0 + 1 < P.sw ? x0 + 1 : P.sw - 1) * P.cn;
+            for (int c = 0; c < nc; ++c) {
+                const int h0 = ((int)r0[o0 + c] * c0 + (int)r0[o1 + c] * c1) >> 4, h1 = ((int)r1[o0 + c] * c0 + (int)r1[o1 + c] * c1) >> 4;
+                v[c] = (((b0 * h0) >> 16) + ((b1 * h1) >> 16) + 2) >> 2;
+            }
+        } else {
+            for (int c = 0; c < nc; ++c) v[c] = r0[(dx4 + i) * P.cn + c];
+        }
+        packed |= (uint32_t)((v[0] * P.k[0] + v[1] * P.k[1] + v[2] * P.k[2] + (1 << 14)) >> 15) << (8 * i);
+    }
+    return packed;
 }
 
 }  // namespace orbdev

@@ -21,6 +21,7 @@
 // | `h->d_po` | carve_scratch | `orbo_pose_optimization_frames` (it calls the two above), `orbv_transform`, `orbp_distinctive_descriptors`, `orbp_update_normal_and_depth`, `orbm_hamming_knn2` |
 // | `orbr_state::d_buf` | carve_scratch | `orbr_submit` (it calls the searches and pose calls above) |
 // | `h->d_xl` | grow_device | the frame blocks of the matcher searches' global-memory form (matcher.cu `launch_proj`) |
+// | `h->d_src` | grow_device | the host camera images of `orbr_submit`'s colour or resized steps (extractor.cu `extract_batch_source`) |
 //
 // Captured CUDA graphs hold pointers into these buffers, so a per-call buffer only grows in an eager call: growth inside a capture is
 // refused.  The exact-size blocks never grow.

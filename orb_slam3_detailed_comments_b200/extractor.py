@@ -24,7 +24,7 @@ class ORBextractor:
         N.check(self._L.orbx_create(C.byref(cfg), C.byref(self._h)))
         self.nfeatures, self.scaleFactor, self.nlevels = nfeatures, scaleFactor, nlevels
         self.iniThFAST, self.minThFAST = iniThFAST, minThFAST
-        self.max_batch = max_batch
+        self.max_batch, self.device = max_batch, device
         sc, isc, s2, is2 = (np.zeros(nlevels, np.float32) for _ in range(4))
         q, um = np.zeros(nlevels, np.int32), np.zeros(16, np.int32)
         N.check(self._L.orbx_get_tables(self._h, N.ptr(sc), N.ptr(isc), N.ptr(s2), N.ptr(is2), N.ptr(q), N.ptr(um)))
@@ -80,14 +80,27 @@ class ORBextractor:
         return mono.value, kps[:n.value].copy(), desc[:n.value].copy()
 
     # ---- batched API ---------------------------------------------------------------------------
-    def extract_batch(self, images, lapping=(0, 0)):
-        """images: (B, H, W) uint8 host array.  Returns (n[B], mono[B]); results stay on the device."""
+    def extract_batch(self, images, lapping=(0, 0), rgb=False, resize=None):
+        """images: (B, H, W) grey or (B, H, W, 3 | 4) colour uint8 host array.  Returns (n[B], mono[B]); results stay on the device.
+        Colour images are converted to grey as Tracking::GrabImage* does: BGR(A) channel order, RGB(A) with rgb=True (mbRGB).
+        resize=(width, height) resizes every image first, as System::Track* does for Settings::newImSize; keypoints are in the
+        coordinates of the resized image.  Colour or resized images go to the device as they are (a torch copy on the handle's
+        device) and are converted there."""
         images = np.ascontiguousarray(images, np.uint8)
-        b, h, w = images.shape
+        b, h, w = images.shape[:3]
         n = np.zeros(b, np.int32)
         mono = np.zeros(b, np.int32)
-        N.check(self._L.orbx_extract_batch(self._h, N.ptr(images), b, w, h, w, h * w, int(lapping[0]), int(lapping[1]),
-                                           N.ptr(n), N.ptr(mono)))
+        if images.ndim == 3 and resize is None:
+            N.check(self._L.orbx_extract_batch(self._h, N.ptr(images), b, w, h, w, h * w, int(lapping[0]), int(lapping[1]),
+                                               N.ptr(n), N.ptr(mono)))
+            return n, mono
+        import torch
+        assert images.ndim == 3 or images.shape[3] in (3, 4), "(B, H, W), (B, H, W, 3) or (B, H, W, 4) expected"
+        fmt = "gray" if images.ndim == 3 else ("rgb" if rgb else "bgr") + ("a" if images.shape[3] == 4 else "")
+        d = torch.from_numpy(images).to(torch.device("cuda", self.device))
+        torch.cuda.current_stream(d.device).synchronize()      # the copy is on torch's stream, the extraction on the handle's
+        self.extract_batch_device(d.data_ptr(), b, *(resize or (w, h)), lapping=lapping, image_format=fmt, src_size=(w, h))
+        N.check(self._L.orbx_counts(self._h, N.ptr(n), N.ptr(mono), None))
         return n, mono
 
     def extract_batch_async(self, images, lapping=(0, 0)):
@@ -98,11 +111,23 @@ class ORBextractor:
         N.check(self._L.orbx_extract_batch(self._h, N.ptr(images), b, w, h, w, h * w, int(lapping[0]), int(lapping[1]),
                                            None, None))
 
-    def extract_batch_device(self, dptr, batch, width, height, stride=None, image_stride=None, lapping=(0, 0)):
-        stride = stride or width
-        image_stride = image_stride or stride * height
-        N.check(self._L.orbx_extract_batch_device(self._h, C.c_void_p(dptr), batch, width, height, stride, image_stride,
-                                                  int(lapping[0]), int(lapping[1])))
+    def extract_batch_device(self, dptr, batch, width, height, stride=None, image_stride=None, lapping=(0, 0), image_format="gray",
+                             src_size=None):
+        """Images already in device memory.  image_format (a key of _native.IMAGE_FORMATS) and src_size=(width, height) of the
+        images at dptr select orbx_extract_batch_device_format: converted to grey and resized to width x height on the device;
+        stride / image_stride then describe the source (default: tight rows of src_size)."""
+        fmt = N.IMAGE_FORMATS[image_format]
+        if fmt == 0 and src_size is None:
+            stride = stride or width
+            image_stride = image_stride or stride * height
+            N.check(self._L.orbx_extract_batch_device(self._h, C.c_void_p(dptr), batch, width, height, stride, image_stride,
+                                                      int(lapping[0]), int(lapping[1])))
+            return
+        sw, sh = src_size or (width, height)
+        stride = stride or sw * N.FORMAT_CHANNELS[fmt]
+        image_stride = image_stride or stride * sh
+        N.check(self._L.orbx_extract_batch_device_format(self._h, C.c_void_p(dptr), batch, width, height, stride, image_stride,
+                                                         int(lapping[0]), int(lapping[1]), fmt, sw, sh))
 
     def counts(self, batch):
         n, mono, off = np.zeros(batch, np.int32), np.zeros(batch, np.int32), np.zeros(batch + 1, np.int32)
