@@ -177,10 +177,33 @@ orb_status orbm_stereo_pair(orbx_handle* left, orbx_handle* right, float bf, flo
                             float* depth, int32_t cap);
 
 /* ------------------------------------------------------------------------------------------------
+ * Frame::ComputeStereoFromRGBD: mvuRight / mvDepth of an RGB-D frame from its registered depth map
+ * ---------------------------------------------------------------------------------------------- */
+
+/* Element type of a depth map: 16-bit unsigned raw sensor units (CV_16U), or 32-bit float (CV_32F). */
+typedef enum { ORB_DEPTH_U16 = 1, ORB_DEPTH_F32 = 2 } orb_depth_format;
+
+/* Image b < n_images of the last extracted batch is an RGB-D frame (extracted with vLappingArea = {0, 0}); its depth map, of the extracted
+ * width x height, is at depth + b * image_stride_bytes, rows stride_bytes apart (0 = tight rows / images).  Per keypoint, as the
+ * reference does for a camera with zero distortion (mvKeysUn = mvKeys):
+ *   Tracking::GrabImageRGBD: d = raw * depth_factor (one float rounding) unless the map is F32 and |depth_factor - 1| <= 1e-5, in which
+ *     case d = raw; depth_factor is Tracking::mDepthMapFactor, the multiplier (1 / the settings' DepthMapFactor);
+ *   Frame::ComputeStereoFromRGBD: d sampled at ((int)y, (int)x); d > 0: mvDepth = d, mvuRight = x - bf / d; else both -1.
+ * Only the sampled pixels are converted.  Results stay on the device, row-aligned with the compact keypoint rows, and are what the
+ * searches, orbo_pose_edges and orbx_pack_keyframe_device read next; orbm_stereo_download returns them; rows of images >= n_images
+ * are not written.  on_device != 0: `depth` is device memory and the call queues one kernel, with no synchronisation or allocation
+ * (graph capture works).  on_device == 0: host memory, copied into a buffer of the handle on its stream (the memory must stay
+ * unchanged until the copy has run, as for orbx_extract_batch).  Refuses with ORB_ERR_INVALID, before queuing anything, a null
+ * handle or map, n_images outside [1, last batch], an unknown format, or a stride shorter than a row (an image stride shorter than
+ * an image) or not a multiple of the element size. */
+orb_status orbm_stereo_rgbd_batch(orbx_handle* h, int32_t n_images, const void* depth, int32_t depth_format, int32_t stride_bytes,
+                                  size_t image_stride_bytes, float depth_factor, int32_t on_device, float bf);
+
+/* ------------------------------------------------------------------------------------------------
  * ORBmatcher::SearchByProjection family  (include/ORBmatcher.h:40-87, src/ORBmatcher.cc), Nleft == -1
  *
  * The frame whose features are searched is an image of the extractor handle's last batch (for a stereo
- * batch: the LEFT image 2p; its mvuRight comes from orbm_stereo_batch when that ran, else -1).  Several
+ * batch: the LEFT image 2p; its mvuRight comes from orbm_stereo_batch or orbm_stereo_rgbd_batch when one ran, else -1).  Several
  * frames are processed per call; frame f uses queries [query_offset[f], query_offset[f+1]).
  * on_device != 0: every array pointer of the query struct and the output pointers are DEVICE memory and
  * the call does not synchronise (except for reading the two small offset tables).
@@ -691,7 +714,7 @@ typedef struct {
 
 typedef struct {
     int32_t n_frames;
-    const uint8_t* images;               /* HOST: 2 * n_frames images (n_frames with monocular) */
+    const uint8_t* images;               /* HOST: 2 * n_frames images (n_frames with monocular or depth_maps) */
     int32_t width, height, stride;       /* stride in bytes between rows */
     size_t image_stride_bytes;           /* between consecutive images */
     float bf, b;                         /* Frame::mbf, Frame::mb */
@@ -716,16 +739,27 @@ typedef struct {
     int32_t src_width, src_height;       /* 0 = width x height */
     int32_t src_stride;                  /* bytes between rows; 0 = src_width x channels */
     size_t src_image_stride_bytes;       /* bytes between images; 0 = src_stride x src_height */
+    /* RGB-D step (depth_maps != NULL; all five zero = as above): what Tracking::GrabImageRGBD -> Frame::Frame(RGB-D) -> Track does per
+       frame for a camera with zero distortion.  Image f is frame f (n_frames images, extracted with vLappingArea = {0, 0}), and HOST
+       depth map f, of width x height, gives its mvuRight / mvDepth as orbm_stereo_rgbd_batch does, in place of ComputeStereoMatches.
+       The searches (any direction), PoseOptimization and the chained flow follow unchanged.  Refused: monocular together with depth
+       maps (ORB_ERR_INVALID), and camera images of another size than width x height (ORB_ERR_UNSUPPORTED: System::TrackRGBD would
+       resize the depth map too, which is not built). */
+    const void* depth_maps;
+    int32_t depth_format;                /* orb_depth_format */
+    int32_t depth_stride;                /* bytes between rows; 0 = width x element size */
+    size_t depth_image_stride_bytes;     /* bytes between maps; 0 = depth_stride x height */
+    float depth_factor;                  /* Tracking::mDepthMapFactor */
 } orbr_step;
 
 typedef struct {                         /* HOST result buffers; any pointer may be NULL (that result is not copied back) */
     int32_t cap_rows;                    /* capacity, in rows, of every per-row / per-edge array below */
     orbx_keypoint* keypoints;            /* compact rows of the whole batch, image after image (mvKeys) */
     uint8_t* descriptors;                /* [rows][32] (mDescriptors) */
-    float* uright;                       /* [rows] mvuRight (left-eye rows; -1 in a monocular step) */
-    float* depth;                        /* [rows] mvDepth (-1 in a monocular step) */
-    int32_t* n;                          /* [2 n_frames] keypoints per image (n_frames in a monocular step) */
-    int32_t* offsets;                    /* [2 n_frames + 1] first row of every image (n_frames + 1 in a monocular step) */
+    float* uright;                       /* [rows] mvuRight (stereo: the left-eye rows hold it; RGB-D: every row; monocular: -1) */
+    float* depth;                        /* [rows] mvDepth (as uright) */
+    int32_t* n;                          /* [2 n_frames] keypoints per image (n_frames in a monocular or RGB-D step) */
+    int32_t* offsets;                    /* [2 n_frames + 1] first row of every image (n_frames + 1 in a monocular or RGB-D step) */
     int32_t* last_feature_match;         /* [rows] as orbm_search_last_frame */
     int32_t* last_nmatches;              /* [n_frames] */
     int32_t* local_match;                /* [nq_local] as orbm_search_local_points */

@@ -17,6 +17,9 @@ SOURCES = ["extractor.cu", "stereo.cu", "matcher.cu", "triangulation.cu", "lba.c
 # k_ingest (the camera-image stage) is a shared object of its own beside the library, which opens it on first use (extractor.cu)
 INGEST_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_ingest.so")
 INGEST_SOURCES = ["ingest.cu"]
+# k_stereo_rgbd (Frame::ComputeStereoFromRGBD) likewise, opened on the first RGB-D batch (stereo.cu)
+RGBD_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_rgbd.so")
+RGBD_SOURCES = ["rgbd.cu"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -28,6 +31,8 @@ KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4
 # orb_image_format of include/orbslam3_b200.h, and the channels of each
 IMAGE_FORMATS = {"gray": 0, "rgb": 1, "bgr": 2, "rgba": 3, "bgra": 4}
 FORMAT_CHANNELS = {0: 1, 1: 3, 2: 3, 3: 4, 4: 4}
+# orb_depth_format of include/orbslam3_b200.h, by the numpy dtype of the map
+DEPTH_FORMATS = {np.dtype(np.uint16): 1, np.dtype(np.float32): 2}
 
 
 class OrbError(RuntimeError):
@@ -35,8 +40,8 @@ class OrbError(RuntimeError):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so and lib/liborbslam3_b200_ingest.so (nvcc cross-compiles
-    on CPU)."""
+    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so and its side objects lib/liborbslam3_b200_ingest.so and
+    lib/liborbslam3_b200_rgbd.so (nvcc cross-compiles on CPU)."""
     deps = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)] + [os.path.join(_PKG, "..", "include", "orbslam3_b200.h"),
                                                                    os.path.abspath(__file__)]   # the recipe itself
     if os.environ.get("ORB_LIB_PATH"):
@@ -44,7 +49,7 @@ def build(force=False, verbose=False):
     newest = max(os.path.getmtime(d) for d in deps)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     os.makedirs(os.path.dirname(LIB_PATH), exist_ok=True)
-    for out, srcs in ((INGEST_LIB_PATH, INGEST_SOURCES), (LIB_PATH, SOURCES)):
+    for out, srcs in ((INGEST_LIB_PATH, INGEST_SOURCES), (RGBD_LIB_PATH, RGBD_SOURCES), (LIB_PATH, SOURCES)):
         if force or not os.path.exists(out) or os.path.getmtime(out) < newest:
             subprocess.check_call([nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", out] +
                                   [os.path.join(_CSRC, s) for s in srcs])
@@ -109,7 +114,8 @@ class orbr_step(C.Structure):
                 ("th_local", C.c_float), ("nnratio_local", C.c_float), ("far_points", C.c_int32), ("th_far", C.c_float),
                 ("pose_optimization", C.c_int32), ("pose", C.c_void_p), ("local_world_pos", C.c_void_p), ("chain", C.POINTER(orbr_chain)),
                 ("monocular", C.c_int32), ("image_format", C.c_int32), ("src_width", C.c_int32), ("src_height", C.c_int32),
-                ("src_stride", C.c_int32), ("src_image_stride_bytes", C.c_size_t)]
+                ("src_stride", C.c_int32), ("src_image_stride_bytes", C.c_size_t), ("depth_maps", C.c_void_p), ("depth_format", C.c_int32),
+                ("depth_stride", C.c_int32), ("depth_image_stride_bytes", C.c_size_t), ("depth_factor", C.c_float)]
 
 
 class orbr_results(C.Structure):
@@ -206,6 +212,7 @@ SIGNATURES = {
     "orbm_stereo_batch": (_I, [_VP, _I, _F, _F]),
     "orbm_stereo_download": (_I, [_VP, _VP, _VP, _I]),
     "orbm_stereo_pair": (_I, [_VP, _VP, _F, _F, _VP, _VP, _I]),
+    "orbm_stereo_rgbd_batch": (_I, [_VP, _I, _VP, _I, _I, C.c_size_t, _F, _I, _F]),
     "orbm_search_local_points": (_I, [_VP, C.POINTER(orbm_camera), C.POINTER(orbm_local_queries), _F, _F, _I, _F, _VP, _VP]),
     "orbm_search_bow": (_I, [_VP, C.POINTER(orbm_bow_queries), _F, _I, _VP, _VP]),
     "orbm_search_initialization": (_I, [_VP, C.POINTER(orbm_camera), C.POINTER(orbm_init_queries), _I, C.c_float, _I, _VP, _VP]),

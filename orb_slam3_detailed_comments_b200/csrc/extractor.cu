@@ -8,6 +8,8 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <map>
+#include <mutex>
 #include <vector>
 
 #include "extractor.h"
@@ -425,7 +427,7 @@ extern "C" void orbx_destroy(orbx_handle* h) {
     cudaSetDevice(h->cfg.device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     orbr_release(h);
-    for (void* p : {h->d_ws, h->d_stage, h->d_po, h->d_xl, h->d_src})
+    for (void* p : {h->d_ws, h->d_stage, h->d_po, h->d_xl, h->d_src, h->d_dmap})
         if (p) cudaFree(p);
     if (h->h_counts) cudaFreeHost(h->h_counts);
     for (int r = 0; r < orbx_handle::kProfRing; ++r)
@@ -598,27 +600,41 @@ extern "C" orb_status orbx_extract_batch_device(orbx_handle* h, const uint8_t* d
 // ---- camera images of any format and size (k_ingest) ----------------------------------------------------------------------------
 static int format_channels(int format) { return format == ORB_FORMAT_GRAY ? 1 : format <= ORB_FORMAT_BGR ? 3 : 4; }
 
-// k_ingest lives in liborbslam3_b200_ingest.so next to this library (csrc/ingest.cu): its launcher, opened once on first use
-typedef cudaError_t (*IngestLaunch)(const orbdev::IngestPlan*, int32_t, int32_t, cudaStream_t);
-static orb_status ingest_launcher(IngestLaunch* out) {
-    static std::string err;
-    static const IngestLaunch fn = []() -> IngestLaunch {
+orb_status side_symbol(const char* file, const char* symbol, const char* stage, void** out) {
+    static std::mutex mu;
+    static std::map<std::string, std::pair<void*, std::string>> opened;   // file:symbol -> the symbol, or why it is missing
+    std::lock_guard<std::mutex> lock(mu);
+    const std::string key = std::string(file) + ":" + symbol;
+    auto it = opened.find(key);
+    if (it == opened.end()) {
+        void* f = nullptr;
+        std::string err;
         Dl_info info;
         if (!dladdr(reinterpret_cast<void*>(&orbx_create), &info) || !info.dli_fname) {
             err = "dladdr failed";
-            return nullptr;
+        } else {
+            const std::string self(info.dli_fname), path = self.substr(0, self.rfind('/') + 1) + file;
+            void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+            f = so ? dlsym(so, symbol) : nullptr;
+            if (!f) {
+                const char* d = dlerror();
+                err = d ? d : path;
+            }
         }
-        const std::string self(info.dli_fname), path = self.substr(0, self.rfind('/') + 1) + "liborbslam3_b200_ingest.so";
-        void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
-        void* f = so ? dlsym(so, "orb_ingest_launch") : nullptr;
-        if (!f) {
-            const char* d = dlerror();
-            err = d ? d : path;
-        }
-        return reinterpret_cast<IngestLaunch>(f);
-    }();
-    *out = fn;
-    return fn ? ORB_OK : set_error(ORB_ERR_UNSUPPORTED, "the camera-image stage is missing (liborbslam3_b200_ingest.so next to the library): " + err);
+        it = opened.emplace(key, std::make_pair(f, err)).first;
+    }
+    *out = it->second.first;
+    return *out ? ORB_OK
+                : set_error(ORB_ERR_UNSUPPORTED, std::string(stage) + " is missing (" + file + " next to the library): " + it->second.second);
+}
+
+// k_ingest lives in liborbslam3_b200_ingest.so next to this library (csrc/ingest.cu)
+typedef cudaError_t (*IngestLaunch)(const orbdev::IngestPlan*, int32_t, int32_t, cudaStream_t);
+static orb_status ingest_launcher(IngestLaunch* out) {
+    void* f = nullptr;
+    const orb_status s = side_symbol("liborbslam3_b200_ingest.so", "orb_ingest_launch", "the camera-image stage", &f);
+    *out = reinterpret_cast<IngestLaunch>(f);
+    return s;
 }
 
 orb_status check_source(ImageSource& src, int w, int hh) {

@@ -20,6 +20,17 @@ orb_status check_source(ImageSource& src, int w, int hh);
 // extractor.cu: a batch of checked HOST images uploaded into the handle's staging block, then orbx_extract_batch_device_format
 orb_status extract_batch_source(struct orbx_handle* h, const uint8_t* imgs, int batch, int w, int hh, const ImageSource& src, int lap0, int lap1);
 
+// extractor.cu: `symbol` of a stage built into a shared object of its own next to this library (`file`, e.g. liborbslam3_b200_ingest.so),
+// so that this library's kernels stay exactly the set tests/golden/sass_fingerprints.json pins.  Opened on first use and kept; a missing
+// object or symbol is ORB_ERR_UNSUPPORTED naming `stage`.
+orb_status side_symbol(const char* file, const char* symbol, const char* stage, void** out);
+
+// Depth maps of RGB-D frames (orbm_stereo_rgbd_batch, orbr_step): orb_depth_format, row and image strides in bytes
+struct DepthSource { int format; int64_t stride; size_t image_stride; };
+// stereo.cu: fills the zero defaults of `d` (tight rows of w elements, tight maps of hh rows) and refuses, before anything is queued, an
+// unknown format or a stride shorter than a row (an image stride shorter than a map, for n_images > 1) or not a multiple of the element
+orb_status check_depth(DepthSource& d, int n_images, int w, int hh);
+
 struct orbx_handle {
     orbx_config cfg{};
     orb::ExtractGeom geom{};
@@ -60,7 +71,7 @@ struct orbx_handle {
     int2* d_taps = nullptr;
     orbx_keypoint* d_kps = nullptr;  // compact results of the last batch
     uint8_t* d_desc = nullptr;
-    float* d_uright = nullptr;       // Frame::mvuRight / mvDepth of the last stereo batch (row-aligned with d_kps)
+    float* d_uright = nullptr;       // Frame::mvuRight / mvDepth of the last stereo or RGB-D batch (row-aligned with d_kps)
     float* d_depth = nullptr;
     int* d_sad = nullptr;
     uint32_t* d_pat = nullptr;       // rBRIEF pattern, 256 packed pairs transposed for k_orient_describe
@@ -94,6 +105,8 @@ struct orbx_handle {
     size_t xl_bytes = 0;
     uint8_t* d_src = nullptr;       // host camera images of extract_batch_source, uploaded for k_ingest
     size_t src_bytes = 0;
+    uint8_t* d_dmap = nullptr;      // host depth maps of orbm_stereo_rgbd_batch, uploaded for k_stereo_rgbd
+    size_t dmap_bytes = 0;
     int smem_optin = 0;             // cudaDevAttrMaxSharedMemoryPerBlockOptin of the handle's device, read on first use
 };
 

@@ -9,7 +9,8 @@
 // (Frame.cc:380) and skips ComputeStereoMatches; everything after the extraction is shared.  orbr_submit returns as soon as
 // everything is queued; orbr_collect waits for the counts, reads back exactly the rows the batch produced and waits once more.
 // Colour or differently sized camera images (orbr_step::image_format, src_*) go up as they are and become grey level-0 images on the
-// device (k_ingest) before the extraction.
+// device (k_ingest) before the extraction.  An RGB-D step (orbr_step::depth_maps) extracts one image per frame with vLappingArea = {0, 0}
+// and takes mvuRight / mvDepth from the raw depth maps (k_stereo_rgbd, orbm_stereo_rgbd_batch) in place of ComputeStereoMatches.
 // A host thread that keeps several handles in flight (submit k+1 .. k+H-1 before collect k) overlaps uploads, kernels and
 // downloads of different handles without more threads.
 #include <string.h>
@@ -129,10 +130,11 @@ void orbr_release(orbx_handle* h) {   // called by orbx_destroy
 
 extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const orbr_step* S) {
     if (!h || !cam || !S || S->n_frames < 1 || !S->images) return set_error(ORB_ERR_INVALID, "bad arguments");
-    const bool mono = S->monocular != 0;
-    const int nf = S->n_frames, nimg = mono ? nf : 2 * nf;   // monocular: image f is frame f; stereo: eyes 2f, 2f + 1
+    const bool mono = S->monocular != 0, rgbd = S->depth_maps != nullptr;
+    if (mono && rgbd) return set_error(ORB_ERR_INVALID, "a step is monocular or RGB-D, not both");
+    const int nf = S->n_frames, nimg = (mono || rgbd) ? nf : 2 * nf;   // monocular, RGB-D: image f is frame f; stereo: eyes 2f, 2f + 1
     if (nimg > h->cfg.max_batch)
-        return set_error(ORB_ERR_INVALID, mono ? "n_frames exceeds the handle's max_batch" : "2 * n_frames exceeds the handle's max_batch");
+        return set_error(ORB_ERR_INVALID, nimg == nf ? "n_frames exceeds the handle's max_batch" : "2 * n_frames exceeds the handle's max_batch");
     if (h->capturing) return set_error(ORB_ERR_INVALID, "orbr_submit cannot run inside a graph capture");
     const orbm_last_queries* QL = S->last;
     const orbm_local_queries* QC = S->local;
@@ -149,6 +151,16 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     const bool ingest = src.format || src.w || src.h || src.stride || src.image_stride;
     if (ingest) {
         const orb_status s = check_source(src, S->width, S->height);
+        if (s != ORB_OK) return s;
+    }
+    DepthSource dsrc{S->depth_format, S->depth_stride, S->depth_image_stride_bytes};
+    if (rgbd) {
+        if (ingest && (src.w != S->width || src.h != S->height))
+            return set_error(ORB_ERR_UNSUPPORTED, "RGB-D camera images of another size than width x height: System::TrackRGBD's resize of the depth "
+                                                  "map is not built");
+        void* fn = nullptr;
+        orb_status s = check_depth(dsrc, nf, S->width, S->height);
+        if (s == ORB_OK) s = side_symbol("liborbslam3_b200_rgbd.so", "orb_rgbd_launch", "the RGB-D depth stage", &fn);
         if (s != ORB_OK) return s;
     }
     ORB_CUDA(cudaSetDevice(h->cfg.device));
@@ -181,11 +193,14 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
     const bool po = S->pose_optimization != 0 || CH != nullptr;
     cudaStream_t st = h->stream;
     // ---- both eyes of every frame through the extractor, then ComputeStereoMatches; or the one image of every monocular frame
-    //      with vLappingArea = {0, 1000} (Frame.cc:380) and no stereo: mvuRight stays -1 for the searches and PoseOptimization ----
+    //      with vLappingArea = {0, 1000} (Frame.cc:380) and no stereo: mvuRight stays -1 for the searches and PoseOptimization; or the
+    //      one image of every RGB-D frame with {0, 0}, then ComputeStereoFromRGBD from its depth map ----
     orb_status s = ingest ? extract_batch_source(h, S->images, nimg, S->width, S->height, src, 0, mono ? 1000 : 0)
                           : orbx_extract_batch(h, S->images, nimg, S->width, S->height, S->stride, S->image_stride_bytes, 0, mono ? 1000 : 0, nullptr, nullptr);
     if (s != ORB_OK) return s;
-    if (!mono && (s = orbm_stereo_batch(h, nf, S->bf, S->b)) != ORB_OK) return s;
+    if (rgbd) s = orbm_stereo_rgbd_batch(h, nf, S->depth_maps, dsrc.format, (int32_t)dsrc.stride, dsrc.image_stride, S->depth_factor, 0, S->bf);
+    else if (!mono) s = orbm_stereo_batch(h, nf, S->bf, S->b);
+    if (s != ORB_OK) return s;
     // ---- the step's device block, carved after the extraction is queued so that only the query copies precede the first search.
     //      The chained flow and the local-map flow share the frame table, offsets, descriptors and world positions of their queries ----
     struct Ptrs {

@@ -22,6 +22,7 @@
 // | `orbr_state::d_buf` | carve_scratch | `orbr_submit` (it calls the searches and pose calls above) |
 // | `h->d_xl` | grow_device | the frame blocks of the matcher searches' global-memory form (matcher.cu `launch_proj`) |
 // | `h->d_src` | grow_device | the host camera images of `orbr_submit`'s colour or resized steps (extractor.cu `extract_batch_source`) |
+// | `h->d_dmap` | grow_device | the host depth maps of `orbm_stereo_rgbd_batch` and of `orbr_submit`'s RGB-D steps (stereo.cu) |
 //
 // Captured CUDA graphs hold pointers into these buffers, so a per-call buffer only grows in an eager call: growth inside a capture is
 // refused.  The exact-size blocks never grow.

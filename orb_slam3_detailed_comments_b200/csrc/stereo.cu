@@ -1,4 +1,5 @@
-// stereo.cu -- Frame::ComputeStereoMatches (/root/reference/src/Frame.cc:1102-1358) on the device.
+// stereo.cu -- Frame::ComputeStereoMatches (/root/reference/src/Frame.cc:1102-1358) on the device, and the host side of
+// Frame::ComputeStereoFromRGBD (its kernel is in csrc/rgbd.cu).
 // One warp per LEFT keypoint: lanes stride over the right image's keypoints (row-band, octave and
 // disparity-range gates, then 256-bit Hamming with __popc), shuffle arg-min with index tie-break
 // (= "first strictly smaller" in ascending right index), 11x11 SAD over 11 shifts on the raw pyramid
@@ -10,6 +11,7 @@
 #include "extractor.h"
 #include "devmath.cuh"
 #include "stereo_core.cuh"
+#include "rgbd_core.cuh"
 
 using namespace orb;
 using namespace orbdev;
@@ -368,4 +370,52 @@ extern "C" orb_status orbm_stereo_pair(orbx_handle* left, orbx_handle* right, fl
     s = orbx_counts(left, nullptr, nullptr, nullptr);
     if (s != ORB_OK) return s;
     return download_stereo_rows(left, image_features(left, 0), uright, depth, cap, "output buffer smaller than N");
+}
+
+// ---- Frame::ComputeStereoFromRGBD: k_stereo_rgbd lives in liborbslam3_b200_rgbd.so next to this library (csrc/rgbd.cu) --------------
+typedef cudaError_t (*RgbdLaunch)(const orbdev::RgbdPlan*, int32_t, int32_t, int32_t, cudaStream_t);
+
+orb_status check_depth(DepthSource& d, int n_images, int w, int hh) {
+    if (d.format != ORB_DEPTH_U16 && d.format != ORB_DEPTH_F32) return set_error(ORB_ERR_INVALID, "unknown depth format");
+    const int64_t elem = d.format == ORB_DEPTH_U16 ? 2 : 4, row = (int64_t)w * elem;
+    if (d.stride == 0) d.stride = row;
+    if (d.image_stride == 0) d.image_stride = (size_t)d.stride * hh;
+    if (d.stride < row || d.stride > INT32_MAX || d.stride % elem || d.image_stride % elem ||
+        (n_images > 1 && d.image_stride < (size_t)d.stride * hh))
+        return set_error(ORB_ERR_INVALID, "depth stride shorter than a row (or a map) or not a multiple of the element size");
+    return ORB_OK;
+}
+
+extern "C" orb_status orbm_stereo_rgbd_batch(orbx_handle* h, int32_t n_images, const void* depth, int32_t depth_format, int32_t stride_bytes,
+                                             size_t image_stride_bytes, float depth_factor, int32_t on_device, float bf) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) return set_error(ORB_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
+    if (!h || !depth) return set_error(ORB_ERR_INVALID, "null handle or depth map");
+    if (n_images < 1 || n_images > h->last_batch) return set_error(ORB_ERR_INVALID, "n_images exceeds the last extracted batch");
+    DepthSource D{depth_format, stride_bytes, image_stride_bytes};
+    orb_status s = check_depth(D, n_images, h->cur_w, h->cur_h);
+    void* fn = nullptr;
+    if (s == ORB_OK) s = side_symbol("liborbslam3_b200_rgbd.so", "orb_rgbd_launch", "the RGB-D depth stage", &fn);
+    if (s != ORB_OK) return s;
+    ORB_CUDA(cudaSetDevice(h->cfg.device));
+    const uint8_t* src = static_cast<const uint8_t*>(depth);
+    if (!on_device) {   // the maps go up tight into the handle's buffer
+        const size_t row = (size_t)h->cur_w * (D.format == ORB_DEPTH_U16 ? 2 : 4), img = row * h->cur_h;
+        if ((s = grow_device(h->dmap_bytes, h->d_dmap, img * n_images, h->capturing)) != ORB_OK) return s;
+        if (D.image_stride == (size_t)D.stride * h->cur_h)   // the whole batch is one pitched 2-D copy
+            ORB_CUDA(cudaMemcpy2DAsync(h->d_dmap, row, src, D.stride, row, (size_t)h->cur_h * n_images, cudaMemcpyHostToDevice, h->stream));
+        else
+            for (int b = 0; b < n_images; ++b)
+                ORB_CUDA(cudaMemcpy2DAsync(h->d_dmap + b * img, row, src + b * D.image_stride, D.stride, row, h->cur_h, cudaMemcpyHostToDevice, h->stream));
+        src = h->d_dmap;
+        D.stride = (int64_t)row;
+        D.image_stride = img;
+    }
+    const orbdev::RgbdPlan P{src, (int64_t)D.image_stride, D.stride, D.format, orbdev::rgbd_scaled(D.format, depth_factor) ? 1 : 0, depth_factor, bf,
+                             h->d_kps, h->d_offsets, h->d_nkp, h->d_uright, h->d_depth};
+    const cudaError_t e = reinterpret_cast<RgbdLaunch>(fn)(&P, n_images, h->geom.kpTotal, h->cfg.device, h->stream);
+    if (e != cudaSuccess) return set_error(ORB_ERR_CUDA, std::string("k_stereo_rgbd: ") + cudaGetErrorString(e));
+    ORB_LAUNCHED();
+    h->stereo_valid = true;
+    return ORB_OK;
 }

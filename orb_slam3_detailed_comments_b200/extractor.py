@@ -188,6 +188,24 @@ class ORBextractor:
         N.check(self._L.orbm_stereo_download(self._h, N.ptr(uR), N.ptr(dep), max(len(uR), 1)))
         return uR[:rows], dep[:rows]
 
+    # ---- Frame::ComputeStereoFromRGBD ---------------------------------------------------------------------------------------
+    def stereo_rgbd_batch(self, depth, depth_factor, bf):
+        """mvuRight / mvDepth of the first len(depth) images of the last batch (RGB-D frames, extracted with lapping (0, 0)) from their
+        depth maps: depth is an (n, H, W) uint16 or float32 host array or CUDA tensor of the extracted size, rows contiguous (any row or
+        image stride); depth_factor is Tracking::mDepthMapFactor (1 / the settings' DepthMapFactor), applied as GrabImageRGBD applies it.
+        Results stay on the device (stereo_download reads them)."""
+        on_device = hasattr(depth, "data_ptr")
+        if on_device:
+            import torch
+            dt = np.dtype({torch.uint16: np.uint16, torch.float32: np.float32}[depth.dtype])
+            ptr, strides = depth.data_ptr(), tuple(s * dt.itemsize for s in depth.stride())
+        else:
+            dt, ptr, strides = depth.dtype, depth.ctypes.data, depth.strides
+        assert depth.ndim == 3 and strides[2] == dt.itemsize, "(n, H, W) maps with contiguous rows expected"
+        fmt = N.DEPTH_FORMATS[dt]
+        N.check(self._L.orbm_stereo_rgbd_batch(self._h, depth.shape[0], C.c_void_p(ptr), fmt, strides[1], strides[0], float(depth_factor),
+                                               1 if on_device else 0, float(bf)))
+
     def stereo_pair(self, right, n_left, bf, b):
         """mvuRight, mvDepth for image 0 of `self` (left eye) against image 0 of `right`."""
         uR = np.zeros(max(n_left, 1), np.float32)

@@ -11,6 +11,8 @@
 
 #define CV_8U 0
 #define CV_8UC1 0
+#define CV_16U 2
+#define CV_32F 5
 
 namespace cv {
 
@@ -38,7 +40,8 @@ class Mat {
     size_t step = 0;
     Mat() {}
     Mat(int r, int c, int /*type*/) { create(r, c, 0); }
-    Mat(int r, int c, int /*type*/, void* ext, size_t stp) : rows(r), cols(c), data((uint8_t*)ext), step(stp) {}
+    // over external data of any element type (a CV_32F depth map: Frame::ComputeStereoFromRGBD); the owning forms are 8-bit only
+    Mat(int r, int c, int type, void* ext, size_t stp) : rows(r), cols(c), data((uint8_t*)ext), step(stp), type_(type) {}
     void create(int r, int c, int /*type*/) {
         rows = r; cols = c; step = (size_t)c;
         store_.reset(new std::vector<uint8_t>((size_t)r * c));
@@ -46,16 +49,17 @@ class Mat {
     }
     void release() { rows = cols = 0; data = nullptr; store_.reset(); }
     bool empty() const { return data == nullptr || rows == 0 || cols == 0; }
-    int type() const { return CV_8UC1; }
+    int type() const { return type_; }
     bool isContinuous() const { return step == (size_t)cols; }
     uint8_t* ptr(int r = 0) { return data + (size_t)r * step; }
     const uint8_t* ptr(int r = 0) const { return data + (size_t)r * step; }
     template <typename T> T* ptr(int r = 0) { return reinterpret_cast<T*>(data + (size_t)r * step); }
     template <typename T> const T* ptr(int r = 0) const { return reinterpret_cast<const T*>(data + (size_t)r * step); }
-    Mat row(int r) const { Mat m; m.rows = 1; m.cols = cols; m.step = step; m.data = data + (size_t)r * step; m.store_ = store_; return m; }
+    Mat row(int r) const { Mat m; m.rows = 1; m.cols = cols; m.step = step; m.data = data + (size_t)r * step; m.type_ = type_; m.store_ = store_; return m; }
     Mat clone() const { Mat m; if (!empty()) { m.create(rows, cols, 0); for (int r = 0; r < rows; ++r) std::memcpy(m.ptr(r), ptr(r), (size_t)cols); } return m; }
 
    private:
+    int type_ = CV_8UC1;
     std::shared_ptr<std::vector<uint8_t>> store_;
 };
 

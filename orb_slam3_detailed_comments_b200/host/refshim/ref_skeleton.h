@@ -306,6 +306,7 @@ class Frame {
    public:
 //@ref Frame.h
     void ComputeStereoMatches();
+    void ComputeStereoFromRGBD(const cv::Mat &imDepth);
     inline Sophus::SE3<float> GetPose() const {
         return mTcw;
     }

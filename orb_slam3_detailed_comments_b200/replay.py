@@ -80,10 +80,12 @@ class TrackingStep:
     one host thread: submit on handles k+1 .. k+H-1 before collecting handle k.  A monocular step takes direction 0 for every
     frame (bMono) and ignores bf / b.  image_format (a key of _native.IMAGE_FORMATS: gray, rgb, bgr, rgba, bgra) is the layout of
     the submitted images, converted to grey on the device as Tracking::GrabImage* does; resize=(width, height) resizes them first on
-    the device, as System::Track* does for Settings::newImSize, and the results are in the coordinates of the resized images."""
+    the device, as System::Track* does for Settings::newImSize, and the results are in the coordinates of the resized images.
+    With rgbd=True each frame is one camera image plus its depth map (submit's depth=), extracted with vLappingArea = {0, 0}; mvuRight /
+    mvDepth come from the map as Frame::ComputeStereoFromRGBD computes them, depth_factor being Tracking::mDepthMapFactor; b is unused."""
 
     def __init__(self, extractor, cam, bf, b, th_last=15.0, th_local=3.0, nnratio_local=0.8, check_orientation=True, far_points=False,
-                 th_far=50.0, monocular=False, image_format="gray", resize=None):
+                 th_far=50.0, monocular=False, image_format="gray", resize=None, rgbd=False, depth_factor=1.0):
         import ctypes as C
         from . import _native as N
         self._C, self._N, self._L = C, N, N.lib()
@@ -91,15 +93,17 @@ class TrackingStep:
         self.args = (float(bf), float(b), float(th_last), 1 if check_orientation else 0, float(th_local), float(nnratio_local),
                      1 if far_points else 0, float(th_far))
         self.monocular = bool(monocular)
+        self.rgbd, self.depth_factor = bool(rgbd), float(depth_factor)
         self.image_format, self.resize = N.IMAGE_FORMATS[image_format], resize
         self._keep = None
 
-    def submit(self, images, last=None, local=None, pose=None, local_world_pos=None, chain=None):
-        """images: (2 * n_frames, H, W[, C]) uint8 host array, (n_frames, H, W[, C]) for a monocular step, C the channels of
+    def submit(self, images, last=None, local=None, pose=None, local_world_pos=None, chain=None, depth=None):
+        """images: (2 * n_frames, H, W[, C]) uint8 host array, (n_frames, H, W[, C]) for a monocular or RGB-D step, C the channels of
         image_format; last / local: dicts of host arrays with the field names of
         orbm_last_queries / orbm_local_queries (fimg, off, Tcw, dir, xw, oct, ang, desc, obs / fimg, off, px, py, pxr, lvl, vc, desc
         [, td, in_view]); pose + local_world_pos switch PoseOptimization on.  chain: dict(off, xw, normal, max_dist, min_dist, desc,
-        last_query[, cos_limit]) of the frames' local map points selects the chained flow (orbr_chain): needs last and pose, no local."""
+        last_query[, cos_limit]) of the frames' local map points selects the chained flow (orbr_chain): needs last and pose, no local.
+        depth: the (n_frames, H', W') uint16 or float32 host depth maps of an RGB-D step, of the extracted size, rows contiguous."""
         C, N = self._C, self._N
         cn = N.FORMAT_CHANNELS[self.image_format]
         assert images.dtype == np.uint8 and images.flags["C_CONTIGUOUS"] and images.shape[3:] == ((cn,) if cn > 1 else ())
@@ -108,7 +112,11 @@ class TrackingStep:
         if self.image_format or self.resize is not None:
             src = (self.image_format, w, h, w * cn, w * h * cn)
             w, h = self.resize or (w, h)
-        nf = nimg if self.monocular else nimg // 2
+        nf = nimg if (self.monocular or self.rgbd) else nimg // 2
+        dsrc = (None, 0, 0, 0, 0.0)
+        if self.rgbd:
+            assert depth is not None and depth.ndim == 3 and depth.strides[2] == depth.itemsize
+            dsrc = (N.ptr(depth), N.DEPTH_FORMATS[depth.dtype], depth.strides[1], depth.strides[0], self.depth_factor)
         bf, b, thl, ori, thc, nnr, far, thfar = self.args
         ql = qc = None
         if last is not None:
@@ -125,8 +133,8 @@ class TrackingStep:
         st = N.orbr_step(nf, N.ptr(images), w, h, w, w * h, bf, b, C.pointer(ql) if ql is not None else None, thl, ori,
                          C.pointer(qc) if qc is not None else None, thc, nnr, far, thfar, 1 if po else 0,
                          N.ptr(pose) if po else None, N.ptr(local_world_pos) if (po and local_world_pos is not None) else None,
-                         C.pointer(ch) if ch is not None else None, 1 if self.monocular else 0, *src)
-        self._keep = (images, last, local, pose, local_world_pos, ql, qc, chain, ch)      # the arrays must outlive the asynchronous copies
+                         C.pointer(ch) if ch is not None else None, 1 if self.monocular else 0, *src, *dsrc)
+        self._keep = (images, last, local, pose, local_world_pos, ql, qc, chain, ch, depth)   # the arrays must outlive the asynchronous copies
         N.check(self._L.orbr_submit(self.ex._h, C.byref(self.cam), C.byref(st)))
 
     def collect(self, out):
