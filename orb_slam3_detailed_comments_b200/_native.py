@@ -14,13 +14,6 @@ _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("ORB_LIB_PATH") or os.path.join(_PKG, "lib", "liborbslam3_b200.so")   # ORB_LIB_PATH: an instrumented build (tools/qt_phases.py)
 SOURCES = ["extractor.cu", "stereo.cu", "matcher.cu", "triangulation.cu", "lba.cu", "poseopt.cu", "bow.cu", "mappoint.cu", "liba.cu", "knn.cu", "replay.cu"]
 
-# k_ingest (the camera-image stage) is a shared object of its own beside the library, which opens it on first use (extractor.cu)
-INGEST_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_ingest.so")
-INGEST_SOURCES = ["ingest.cu"]
-# k_stereo_rgbd (Frame::ComputeStereoFromRGBD) likewise, opened on the first RGB-D batch (stereo.cu)
-RGBD_LIB_PATH = os.path.join(_PKG, "lib", "liborbslam3_b200_rgbd.so")
-RGBD_SOURCES = ["rgbd.cu"]
-
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
@@ -40,19 +33,17 @@ class OrbError(RuntimeError):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so and its side objects lib/liborbslam3_b200_ingest.so and
-    lib/liborbslam3_b200_rgbd.so (nvcc cross-compiles on CPU)."""
+    """Compile every CUDA source for sm_90a into lib/liborbslam3_b200.so (nvcc cross-compiles on CPU)."""
     deps = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)] + [os.path.join(_PKG, "..", "include", "orbslam3_b200.h"),
                                                                    os.path.abspath(__file__)]   # the recipe itself
     if os.environ.get("ORB_LIB_PATH"):
         return LIB_PATH                       # an explicitly chosen build is never rebuilt
-    newest = max(os.path.getmtime(d) for d in deps)
+    if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
+        return LIB_PATH
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     os.makedirs(os.path.dirname(LIB_PATH), exist_ok=True)
-    for out, srcs in ((INGEST_LIB_PATH, INGEST_SOURCES), (RGBD_LIB_PATH, RGBD_SOURCES), (LIB_PATH, SOURCES)):
-        if force or not os.path.exists(out) or os.path.getmtime(out) < newest:
-            subprocess.check_call([nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", out] +
-                                  [os.path.join(_CSRC, s) for s in srcs])
+    subprocess.check_call([nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB_PATH] +
+                          [os.path.join(_CSRC, s) for s in SOURCES])
     return LIB_PATH
 
 

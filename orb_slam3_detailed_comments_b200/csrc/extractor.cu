@@ -1,15 +1,12 @@
 // extractor.cu -- host side of the batched ORB extractor + its C ABI (include/orbslam3_b200.h).
 // Replaces ORBextractor::ORBextractor / operator() / ComputePyramid / ComputeKeyPointsOctTree
 // (/root/reference/src/ORBextractor.cc:468-571, 1557-1682, 1687-1738, 1061-1208).
-#include <dlfcn.h>
 #include <math.h>
 #include <string.h>
 
 #include <stdlib.h>
 
 #include <algorithm>
-#include <map>
-#include <mutex>
 #include <vector>
 
 #include "extractor.h"
@@ -569,30 +566,49 @@ static orb_status check_batch_args(orbx_handle* h, const void* imgs, int batch, 
     return apply_geometry(h, w, hh);
 }
 
+// The profiling ring: the next slot's stage events, the batch's first one recorded now
+static void profile_batch(orbx_handle* h) {
+    if (!h->profiling) return;
+    h->ev = h->evr[h->prof_count % orbx_handle::kProfRing];
+    ++h->prof_count;
+    cudaEventRecord(h->ev[0], h->stream);
+}
+
+// Level 0 of w x hh images in the handle's own pyramid block, rows padded to 16 bytes
+static const LevelGeom& own_level0(orbx_handle* h, int w, int hh) {
+    LevelGeom& L0 = h->geom.lv[0];
+    L0.base = h->d_pyr;
+    L0.pitch = round_up(w, 16);
+    L0.img_stride = (int64_t)L0.pitch * hh;
+    return L0;
+}
+
+orb_status copy_images(orbx_handle* h, uint8_t* dst, size_t dst_pitch, const uint8_t* src, size_t src_pitch, size_t src_image, size_t row,
+                       int rows, int batch, cudaMemcpyKind kind) {
+    if (src_image == src_pitch * rows)
+        ORB_CUDA(cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, row, (size_t)rows * batch, kind, h->stream));
+    else
+        for (int b = 0; b < batch; ++b)
+            ORB_CUDA(cudaMemcpy2DAsync(dst + b * dst_pitch * rows, dst_pitch, src + b * src_image, src_pitch, row, rows, kind, h->stream));
+    return ORB_OK;
+}
+
 extern "C" orb_status orbx_extract_batch_device(orbx_handle* h, const uint8_t* d_imgs, int32_t batch, int32_t w,
                                                 int32_t hh, int32_t stride, size_t image_stride_bytes, int32_t lap0,
                                                 int32_t lap1) {
     orb_status s = check_batch_args(h, d_imgs, batch, w, hh, stride);
     if (s != ORB_OK) return s;
-    LevelGeom& L0 = h->geom.lv[0];
-    if (h->profiling) {
-        h->ev = h->evr[h->prof_count % orbx_handle::kProfRing];
-        ++h->prof_count;
-        cudaEventRecord(h->ev[0], h->stream);
-    }
+    profile_batch(h);
     const bool aligned = ((uintptr_t)d_imgs % 16 == 0) && (stride % 8 == 0) && (image_stride_bytes % 8 == 0);   // k_fast_cells_v2 stages with 64-bit loads
-    uint8_t* own = h->d_pyr;  // level 0 block of the handle
     if (aligned) {
+        LevelGeom& L0 = h->geom.lv[0];
         L0.base = const_cast<uint8_t*>(d_imgs);
         L0.pitch = stride;
         L0.img_stride = (int64_t)image_stride_bytes;
     } else {
-        L0.base = own;
-        L0.pitch = round_up(w, 16);
-        L0.img_stride = (int64_t)L0.pitch * hh;
-        for (int b = 0; b < batch; ++b)
-            ORB_CUDA(cudaMemcpy2DAsync(own + (size_t)b * L0.img_stride, L0.pitch, d_imgs + (size_t)b * image_stride_bytes,
-                                       stride, w, hh, cudaMemcpyDeviceToDevice, h->stream));
+        const LevelGeom& L0 = own_level0(h, w, hh);
+        s = copy_images(h, L0.base, L0.pitch, d_imgs, stride, image_stride_bytes, w, hh, batch, cudaMemcpyDeviceToDevice);
+        if (s != ORB_OK) return s;
     }
     return run_pipeline(h, batch, lap0, lap1);
 }
@@ -600,42 +616,18 @@ extern "C" orb_status orbx_extract_batch_device(orbx_handle* h, const uint8_t* d
 // ---- camera images of any format and size (k_ingest) ----------------------------------------------------------------------------
 static int format_channels(int format) { return format == ORB_FORMAT_GRAY ? 1 : format <= ORB_FORMAT_BGR ? 3 : 4; }
 
-orb_status side_symbol(const char* file, const char* symbol, const char* stage, void** out) {
-    static std::mutex mu;
-    static std::map<std::string, std::pair<void*, std::string>> opened;   // file:symbol -> the symbol, or why it is missing
-    std::lock_guard<std::mutex> lock(mu);
-    const std::string key = std::string(file) + ":" + symbol;
-    auto it = opened.find(key);
-    if (it == opened.end()) {
-        void* f = nullptr;
-        std::string err;
-        Dl_info info;
-        if (!dladdr(reinterpret_cast<void*>(&orbx_create), &info) || !info.dli_fname) {
-            err = "dladdr failed";
-        } else {
-            const std::string self(info.dli_fname), path = self.substr(0, self.rfind('/') + 1) + file;
-            void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
-            f = so ? dlsym(so, symbol) : nullptr;
-            if (!f) {
-                const char* d = dlerror();
-                err = d ? d : path;
-            }
-        }
-        it = opened.emplace(key, std::make_pair(f, err)).first;
-    }
-    *out = it->second.first;
-    return *out ? ORB_OK
-                : set_error(ORB_ERR_UNSUPPORTED, std::string(stage) + " is missing (" + file + " next to the library): " + it->second.second);
+namespace orb {
+
+// colour conversion and resize of a batch of camera images into level 0 (resize_core.cuh ig_pixels4).  256 threads cover 1024 px x
+// 1 row; blockIdx.z is the image.
+__global__ void __launch_bounds__(256) k_ingest(const __grid_constant__ orbdev::IngestPlan P) {
+    const int dx4 = 4 * (blockIdx.x * 256 + threadIdx.x), dy = blockIdx.y;
+    if (dx4 >= P.dw) return;
+    const uint32_t v = orbdev::ig_pixels4(P, P.src + (int64_t)blockIdx.z * P.src_image, dx4, dy);
+    *reinterpret_cast<uint32_t*>(P.dst + (int64_t)blockIdx.z * P.dst_image + (int64_t)dy * P.dpitch + dx4) = v;
 }
 
-// k_ingest lives in liborbslam3_b200_ingest.so next to this library (csrc/ingest.cu)
-typedef cudaError_t (*IngestLaunch)(const orbdev::IngestPlan*, int32_t, int32_t, cudaStream_t);
-static orb_status ingest_launcher(IngestLaunch* out) {
-    void* f = nullptr;
-    const orb_status s = side_symbol("liborbslam3_b200_ingest.so", "orb_ingest_launch", "the camera-image stage", &f);
-    *out = reinterpret_cast<IngestLaunch>(f);
-    return s;
-}
+}  // namespace orb
 
 orb_status check_source(ImageSource& src, int w, int hh) {
     if (src.format < ORB_FORMAT_GRAY || src.format > ORB_FORMAT_BGRA) return set_error(ORB_ERR_INVALID, "unknown image format");
@@ -652,23 +644,15 @@ extern "C" orb_status orbx_extract_batch_device_format(orbx_handle* h, const uin
                                                        int32_t format, int32_t src_width, int32_t src_height) {
     ImageSource src{format, src_width, src_height, stride, image_stride_bytes};
     if (!h) return set_error(ORB_ERR_INVALID, "null handle");
-    IngestLaunch launch = nullptr;
     orb_status s = check_source(src, w, hh);
-    if (s == ORB_OK) s = ingest_launcher(&launch);
     if (s == ORB_OK) s = check_batch_args(h, d_imgs, batch, w, hh, w);
     if (s != ORB_OK) return s;
-    LevelGeom& L0 = h->geom.lv[0];
-    L0.base = h->d_pyr;
-    L0.pitch = round_up(w, 16);
-    L0.img_stride = (int64_t)L0.pitch * hh;
-    if (h->profiling) {
-        h->ev = h->evr[h->prof_count % orbx_handle::kProfRing];
-        ++h->prof_count;
-        cudaEventRecord(h->ev[0], h->stream);
-    }
+    const LevelGeom& L0 = own_level0(h, w, hh);
+    profile_batch(h);
     const orbdev::IngestPlan P = orbdev::ig_plan(d_imgs, (int64_t)src.image_stride, format, src.w, src.h, (int)src.stride, L0.base, L0.img_stride,
                                                  w, hh, L0.pitch);
-    const cudaError_t e = launch(&P, batch, h->cfg.device, h->stream);
+    k_ingest<<<dim3((P.dw + 1023) / 1024, P.dh, batch), 256, 0, h->stream>>>(P);
+    const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(ORB_ERR_CUDA, std::string("k_ingest: ") + cudaGetErrorString(e));
     ORB_LAUNCHED();
     return run_pipeline(h, batch, lap0, lap1);
@@ -678,17 +662,11 @@ orb_status extract_batch_source(orbx_handle* h, const uint8_t* imgs, int batch, 
     if (!imgs || batch < 1 || batch > h->cfg.max_batch) return set_error(ORB_ERR_INVALID, "bad batch");
     if (w < 1 || hh < 1 || w > h->cfg.max_width || hh > h->cfg.max_height)
         return set_error(ORB_ERR_INVALID, "image larger than the handle's max_width/max_height");
-    IngestLaunch launch = nullptr;
-    if (ingest_launcher(&launch) != ORB_OK) return ORB_ERR_UNSUPPORTED;   // before the upload
     const size_t row = (size_t)src.w * format_channels(src.format), img = row * src.h;
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     orb_status s = grow_device(h->src_bytes, h->d_src, img * batch, h->capturing);
+    if (s == ORB_OK) s = copy_images(h, h->d_src, row, imgs, src.stride, src.image_stride, row, src.h, batch, cudaMemcpyHostToDevice);
     if (s != ORB_OK) return s;
-    if (src.image_stride == (size_t)src.stride * src.h)   // the whole batch is one pitched 2-D copy
-        ORB_CUDA(cudaMemcpy2DAsync(h->d_src, row, imgs, src.stride, row, (size_t)src.h * batch, cudaMemcpyHostToDevice, h->stream));
-    else
-        for (int b = 0; b < batch; ++b)
-            ORB_CUDA(cudaMemcpy2DAsync(h->d_src + b * img, row, imgs + b * src.image_stride, src.stride, row, src.h, cudaMemcpyHostToDevice, h->stream));
     return orbx_extract_batch_device_format(h, h->d_src, batch, w, hh, (int)row, img, lap0, lap1, src.format, src.w, src.h);
 }
 
@@ -697,24 +675,10 @@ extern "C" orb_status orbx_extract_batch(orbx_handle* h, const uint8_t* imgs, in
                                          int32_t* n_out, int32_t* mono_index) {
     orb_status s = check_batch_args(h, imgs, batch, w, hh, stride);
     if (s != ORB_OK) return s;
-    LevelGeom& L0 = h->geom.lv[0];
-    L0.base = h->d_pyr;
-    L0.pitch = round_up(w, 16);
-    L0.img_stride = (int64_t)L0.pitch * hh;
-    if (h->profiling) {
-        h->ev = h->evr[h->prof_count % orbx_handle::kProfRing];
-        ++h->prof_count;
-        cudaEventRecord(h->ev[0], h->stream);
-    }
-    if (image_stride_bytes == (size_t)stride * hh) {
-        // the whole batch is one pitched 2-D copy: rows = batch * height
-        ORB_CUDA(cudaMemcpy2DAsync(L0.base, L0.pitch, imgs, stride, w, (size_t)hh * batch, cudaMemcpyHostToDevice, h->stream));
-    } else {
-        for (int b = 0; b < batch; ++b)
-            ORB_CUDA(cudaMemcpy2DAsync(L0.base + (size_t)b * L0.img_stride, L0.pitch, imgs + (size_t)b * image_stride_bytes,
-                                       stride, w, hh, cudaMemcpyHostToDevice, h->stream));
-    }
-    s = run_pipeline(h, batch, lap0, lap1);
+    const LevelGeom& L0 = own_level0(h, w, hh);
+    profile_batch(h);
+    s = copy_images(h, L0.base, L0.pitch, imgs, stride, image_stride_bytes, w, hh, batch, cudaMemcpyHostToDevice);
+    if (s == ORB_OK) s = run_pipeline(h, batch, lap0, lap1);
     if (s != ORB_OK) return s;
     if (n_out || mono_index) {
         s = orbx_counts(h, n_out, mono_index, nullptr);

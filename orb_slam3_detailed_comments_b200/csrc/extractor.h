@@ -20,10 +20,11 @@ orb_status check_source(ImageSource& src, int w, int hh);
 // extractor.cu: a batch of checked HOST images uploaded into the handle's staging block, then orbx_extract_batch_device_format
 orb_status extract_batch_source(struct orbx_handle* h, const uint8_t* imgs, int batch, int w, int hh, const ImageSource& src, int lap0, int lap1);
 
-// extractor.cu: `symbol` of a stage built into a shared object of its own next to this library (`file`, e.g. liborbslam3_b200_ingest.so),
-// so that this library's kernels stay exactly the set tests/golden/sass_fingerprints.json pins.  Opened on first use and kept; a missing
-// object or symbol is ORB_ERR_UNSUPPORTED naming `stage`.
-orb_status side_symbol(const char* file, const char* symbol, const char* stage, void** out);
+// extractor.cu: queues on the handle's stream the copy of `batch` images of `rows` rows of `row` bytes, from `src` (row pitch `src_pitch`,
+// image stride `src_image`) to tight images at `dst` (row pitch `dst_pitch`, image stride dst_pitch x rows): one 2-D copy when the source
+// images are tight too, else one per image
+orb_status copy_images(struct orbx_handle* h, uint8_t* dst, size_t dst_pitch, const uint8_t* src, size_t src_pitch, size_t src_image, size_t row,
+                       int rows, int batch, cudaMemcpyKind kind);
 
 // Depth maps of RGB-D frames (orbm_stereo_rgbd_batch, orbr_step): orb_depth_format, row and image strides in bytes
 struct DepthSource { int format; int64_t stride; size_t image_stride; };

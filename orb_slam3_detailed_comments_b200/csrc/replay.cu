@@ -158,9 +158,7 @@ extern "C" orb_status orbr_submit(orbx_handle* h, const orbm_camera* cam, const 
         if (ingest && (src.w != S->width || src.h != S->height))
             return set_error(ORB_ERR_UNSUPPORTED, "RGB-D camera images of another size than width x height: System::TrackRGBD's resize of the depth "
                                                   "map is not built");
-        void* fn = nullptr;
-        orb_status s = check_depth(dsrc, nf, S->width, S->height);
-        if (s == ORB_OK) s = side_symbol("liborbslam3_b200_rgbd.so", "orb_rgbd_launch", "the RGB-D depth stage", &fn);
+        const orb_status s = check_depth(dsrc, nf, S->width, S->height);
         if (s != ORB_OK) return s;
     }
     ORB_CUDA(cudaSetDevice(h->cfg.device));

@@ -1,5 +1,5 @@
 // rgbd_core.cuh -- one keypoint of Frame::ComputeStereoFromRGBD over a raw depth map, with Tracking::GrabImageRGBD's conversion of the
-// sampled pixel only.  The identical source runs as k_stereo_rgbd's per-thread body (csrc/rgbd.cu) and on the host
+// sampled pixel only.  The identical source runs as k_stereo_rgbd's per-thread body (csrc/stereo.cu) and on the host
 // (tests/host_emul/rgbd_emul.cpp, against a numpy restatement and the oracle).
 #pragma once
 #include "../../include/orbslam3_b200.h"

@@ -1,5 +1,4 @@
-// stereo.cu -- Frame::ComputeStereoMatches (/root/reference/src/Frame.cc:1102-1358) on the device, and the host side of
-// Frame::ComputeStereoFromRGBD (its kernel is in csrc/rgbd.cu).
+// stereo.cu -- Frame::ComputeStereoMatches (/root/reference/src/Frame.cc:1102-1358) and Frame::ComputeStereoFromRGBD on the device.
 // One warp per LEFT keypoint: lanes stride over the right image's keypoints (row-band, octave and
 // disparity-range gates, then 256-bit Hamming with __popc), shuffle arg-min with index tie-break
 // (= "first strictly smaller" in ascending right index), 11x11 SAD over 11 shifts on the raw pyramid
@@ -372,8 +371,23 @@ extern "C" orb_status orbm_stereo_pair(orbx_handle* left, orbx_handle* right, fl
     return download_stereo_rows(left, image_features(left, 0), uright, depth, cap, "output buffer smaller than N");
 }
 
-// ---- Frame::ComputeStereoFromRGBD: k_stereo_rgbd lives in liborbslam3_b200_rgbd.so next to this library (csrc/rgbd.cu) --------------
-typedef cudaError_t (*RgbdLaunch)(const orbdev::RgbdPlan*, int32_t, int32_t, int32_t, cudaStream_t);
+// ---- Frame::ComputeStereoFromRGBD ----------------------------------------------------------------------------------------------------
+namespace orb {
+
+// One thread per keypoint row of each image (rgbd_core.cuh rgbd_row); blockIdx.y is the image.  Only the sampled depth pixels are
+// read and converted.
+__global__ void __launch_bounds__(128) k_stereo_rgbd(const __grid_constant__ orbdev::RgbdPlan P) {
+    const int img = blockIdx.y, i = blockIdx.x * 128 + threadIdx.x;
+    if (i >= P.nkp[img]) return;
+    const int row = P.offsets[img] + i;
+    const float x = P.kps[row].x, y = P.kps[row].y;
+    float u, d;
+    orbdev::rgbd_row(P.depth + (int64_t)img * P.image_stride, P.stride, P.format, P.scaled != 0, P.factor, x, y, P.bf, &u, &d);
+    P.uright[row] = u;
+    P.depth_out[row] = d;
+}
+
+}  // namespace orb
 
 orb_status check_depth(DepthSource& d, int n_images, int w, int hh) {
     if (d.format != ORB_DEPTH_U16 && d.format != ORB_DEPTH_F32) return set_error(ORB_ERR_INVALID, "unknown depth format");
@@ -394,26 +408,21 @@ extern "C" orb_status orbm_stereo_rgbd_batch(orbx_handle* h, int32_t n_images, c
     if (n_images < 1 || n_images > h->last_batch) return set_error(ORB_ERR_INVALID, "n_images exceeds the last extracted batch");
     DepthSource D{depth_format, stride_bytes, image_stride_bytes};
     orb_status s = check_depth(D, n_images, h->cur_w, h->cur_h);
-    void* fn = nullptr;
-    if (s == ORB_OK) s = side_symbol("liborbslam3_b200_rgbd.so", "orb_rgbd_launch", "the RGB-D depth stage", &fn);
     if (s != ORB_OK) return s;
     ORB_CUDA(cudaSetDevice(h->cfg.device));
     const uint8_t* src = static_cast<const uint8_t*>(depth);
     if (!on_device) {   // the maps go up tight into the handle's buffer
         const size_t row = (size_t)h->cur_w * (D.format == ORB_DEPTH_U16 ? 2 : 4), img = row * h->cur_h;
         if ((s = grow_device(h->dmap_bytes, h->d_dmap, img * n_images, h->capturing)) != ORB_OK) return s;
-        if (D.image_stride == (size_t)D.stride * h->cur_h)   // the whole batch is one pitched 2-D copy
-            ORB_CUDA(cudaMemcpy2DAsync(h->d_dmap, row, src, D.stride, row, (size_t)h->cur_h * n_images, cudaMemcpyHostToDevice, h->stream));
-        else
-            for (int b = 0; b < n_images; ++b)
-                ORB_CUDA(cudaMemcpy2DAsync(h->d_dmap + b * img, row, src + b * D.image_stride, D.stride, row, h->cur_h, cudaMemcpyHostToDevice, h->stream));
+        if ((s = copy_images(h, h->d_dmap, row, src, D.stride, D.image_stride, row, h->cur_h, n_images, cudaMemcpyHostToDevice)) != ORB_OK) return s;
         src = h->d_dmap;
         D.stride = (int64_t)row;
         D.image_stride = img;
     }
     const orbdev::RgbdPlan P{src, (int64_t)D.image_stride, D.stride, D.format, orbdev::rgbd_scaled(D.format, depth_factor) ? 1 : 0, depth_factor, bf,
                              h->d_kps, h->d_offsets, h->d_nkp, h->d_uright, h->d_depth};
-    const cudaError_t e = reinterpret_cast<RgbdLaunch>(fn)(&P, n_images, h->geom.kpTotal, h->cfg.device, h->stream);
+    k_stereo_rgbd<<<dim3((h->geom.kpTotal + 127) / 128, n_images), 128, 0, h->stream>>>(P);
+    const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(ORB_ERR_CUDA, std::string("k_stereo_rgbd: ") + cudaGetErrorString(e));
     ORB_LAUNCHED();
     h->stereo_valid = true;

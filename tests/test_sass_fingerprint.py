@@ -3,7 +3,8 @@ tests/golden/sass_fingerprints.json is taken (scripts/sass_fingerprint.py) from 
 (every kernel has had a device run: UNPROVEN is empty).  An intentional kernel change must come with a GPU run and a
 refreshed fingerprint file; an unintentional one (a shared header edit that changes another kernel's code) fails here first.
 Next to the fingerprints, the properties a few kernels were built for are checked in their own SASS: both passes of the tensor-core
-blur run as u8 IMMA, and the 64-bit quadtree and the matcher's global-memory form keep to their GPU-validated local-memory use."""
+blur run as u8 IMMA, and the 64-bit quadtree, the camera-image and RGB-D depth stages and the matcher's global-memory form keep to their
+GPU-validated local-memory use."""
 import importlib.util
 import json
 import os
@@ -74,6 +75,14 @@ def test_k64_quadtree_uses_no_local_memory(ops):
     k = ops["_ZN3orb17k_quadtree_v1_k64ILi512ELi1EEEvNS_11ExtractGeomEiiPKjPKiPjPcliiiS6_PiS8_"]
     assert any(op.startswith("BAR.SYNC") for op in k)
     assert local_ops(k) == 0
+
+
+def test_k_ingest_uses_no_local_memory(ops):
+    assert local_ops(ops["_ZN3orb8k_ingestEN6orbdev10IngestPlanE"]) == 0
+
+
+def test_k_stereo_rgbd_uses_no_local_memory(ops):
+    assert local_ops(ops["_ZN3orb13k_stereo_rgbdEN6orbdev8RgbdPlanE"]) == 0
 
 
 def test_global_form_adds_no_local_memory(ops):
