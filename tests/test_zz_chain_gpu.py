@@ -2,169 +2,35 @@
 Sophus::SE3f -> Frame::isInFrustum of the local map -> SearchByProjection(F, local map points) -> PoseOptimization over every map
 point of the frame; Tracking.cc:3389-3522, 4010-4062) against the CPU oracle, stage by stage.  Integer stages (matches, claims,
 skips, levels, in-view flags) and every float32 value of isInFrustum must be identical; the two optimised poses agree with the fp64
-oracle to 1e-4 like tests/test_poseopt_gpu.py (the device's own first pose is what the later oracle stages start from)."""
+oracle to 1e-4 like tests/test_poseopt_gpu.py (the device's own first pose is what the later oracle stages start from).  The walk is
+tests/_tracking.py's; the monocular and RGB-D forms are in tests/test_zz_mono_step_gpu.py and tests/test_zz_rgbd_step_gpu.py."""
 import numpy as np
 import pytest
 
+from _tracking import run_chained_flow
 from orb_slam3_detailed_comments_b200 import ORBextractor, camera, synth, replay
-from orb_slam3_detailed_comments_b200._native import KP_DTYPE
-from oracle import pyoracle as po
 
 pytestmark = pytest.mark.gpu
 W, H, NF = 640, 480, 1200
 FX, FY, CX, CY, BF, B = 435.2, 435.2, 320.0, 240.0, 47.9, 0.11
-CAM6 = np.float32([FX, FY, CX, CY, BF, B])
-BOUNDS = np.float32([0, W, 0, H])
-f32 = np.float32
-
-
-def _se3f_from_pose(p7):
-    """Optimizer.cc:406-410 + Sophus::SO3f normalisation + Frame::UpdatePoseMatrices, float32 operation by operation."""
-    q = p7[:4].astype(f32)
-    t = p7[4:].astype(f32)
-    ln = f32(np.sqrt(f32(f32(f32(q[0] * q[0]) + f32(q[2] * q[2])) + f32(f32(q[1] * q[1]) + f32(q[3] * q[3])))))
-    q = (q / ln).astype(f32)
-    x, y, z, w = q
-    t2x, t2y, t2z = f32(2) * x, f32(2) * y, f32(2) * z
-    twx, twy, twz = f32(t2x * w), f32(t2y * w), f32(t2z * w)
-    txx, txy, txz, tyy, tyz, tzz = f32(t2x * x), f32(t2y * x), f32(t2z * x), f32(t2y * y), f32(t2z * y), f32(t2z * z)
-    R = np.array([f32(1) - f32(tyy + tzz), f32(txy - twz), f32(txz + twy), f32(txy + twz), f32(1) - f32(txx + tzz), f32(tyz - twx),
-                  f32(txz - twy), f32(tyz + twx), f32(1) - f32(txx + tyy)], f32).reshape(3, 3)
-    i = np.array([-x, -y, -z], f32)
-    p = (t * f32(-1)).astype(f32)
-    uv = np.array([f32(i[1] * p[2]) - f32(i[2] * p[1]), f32(i[2] * p[0]) - f32(i[0] * p[2]), f32(i[0] * p[1]) - f32(i[1] * p[0])], f32)
-    u = (uv + uv).astype(f32)
-    c = np.array([f32(i[1] * u[2]) - f32(i[2] * u[1]), f32(i[2] * u[0]) - f32(i[0] * u[2]), f32(i[0] * u[1]) - f32(i[1] * u[0])], f32)
-    Ow = np.array([f32(f32(p[k] + f32(w * u[k])) + c[k]) for k in range(3)], f32)
-    return np.concatenate([q, t]).astype(f32), R, t, Ow
 
 
 def test_chained_frame_flow_matches_the_oracle_stage_by_stage():
     P = 2
-    rng = np.random.default_rng(5)
-    cam = camera(FX, FY, CX, CY, BF, B, W, H)
     imgs = np.stack([im for p in range(P) for im in synth.stereo_pair(W, H, seed=400 + p)[:2]])
     ex = ORBextractor(NF, 1.2, 8, 20, 7, max_width=W, max_height=H, max_batch=2 * P)
     ex.extract_batch(imgs)
     ex.stereo_batch(P, BF, B)
-    n, _, off, kps, desc = ex.download(2 * P)
+    _, _, off, kps, desc = ex.download(2 * P)
     uR, dep = ex.stereo_download(int(off[-1]))
-    sf = ex.GetScaleFactors()
-    isg = ex.GetInverseScaleSigmaSquares()
-    Tpred = np.tile(np.array([0.0005, -0.0008, 0.0003, 1, 0.004, -0.003, 0.002], np.float32), (P, 1))
-    Tpred[:, :4] /= np.linalg.norm(Tpred[:, :4], axis=1)[:, None]
-    last = dict(off=[0], xw=[], oct=[], ang=[], desc=[], obs=[])
-    ch = dict(off=[0], xw=[], normal=[], max_dist=[], min_dist=[], desc=[], last_query=[])
-    per = []
-    for p in range(P):
+    frames = []
+    for p in range(P):              # the LastFrame and local-map points are the features with a stereo depth; frame p is image 2p
         a, b = int(off[2 * p]), int(off[2 * p + 1])
-        k, d, z, ur = kps[a:b], desc[a:b], dep[a:b], uR[a:b]
-        st = np.nonzero(z > 0)[0]
-        selL, selB = st[::2], st[1::2]
-        pts = lambda s: np.stack([(k["x"][s] - CX) * z[s] / FX, (k["y"][s] - CY) * z[s] / FY, z[s]], 1).astype(np.float32)
-        xwL = pts(selL)
-        gross = rng.random(len(selL)) < 0.06                      # map points at half their depth: same pixel, so the search matches them; the
-        xwL[gross] *= np.float32(0.5)                             # stereo residual then makes PoseOptimization throw them out
-        last["xw"].append(xwL); last["oct"].append(k["octave"][selL].astype(np.int32)); last["ang"].append(k["angle"][selL].astype(np.float32))
-        last["desc"].append(d[selL]); last["obs"].append((rng.random(len(selL)) < 0.9).astype(np.uint8)); last["off"].append(last["off"][-1] + len(selL))
-        # local map: the LastFrame map points themselves (in a shuffled order), points seen by other features, points out of view
-        nC = 200
-        xwB = pts(selB)
-        xwC = np.stack([rng.uniform(-30, 30, nC), rng.uniform(-20, 20, nC), rng.uniform(-10, 40, nC)], 1).astype(np.float32)
-        xw = np.concatenate([xwL, xwB, xwC])
-        dsc = np.concatenate([d[selL], d[selB], rng.integers(0, 256, (nC, 32), dtype=np.uint8)])
-        lq = np.concatenate([np.arange(len(selL)), np.full(len(selB) + nC, -1)]).astype(np.int32)
-        octs = np.concatenate([k["octave"][selL], k["octave"][selB], rng.integers(0, 8, nC)])
-        dist = np.linalg.norm(xw, axis=1).astype(np.float32)
-        maxd = (dist * sf[octs] * rng.uniform(0.75, 1.3, len(xw))).astype(np.float32)
-        nrm = xw / np.maximum(dist[:, None], 1e-6) + rng.normal(0, 0.35, xw.shape)     # MapPoint::mNormalVector: mean viewing direction, camera -> point
-        nrm = (nrm / np.linalg.norm(nrm, axis=1)[:, None]).astype(np.float32)
-        perm = rng.permutation(len(xw))
-        ch["xw"].append(xw[perm]); ch["normal"].append(nrm[perm]); ch["max_dist"].append(maxd[perm]); ch["min_dist"].append((maxd / sf[7]).astype(np.float32)[perm])
-        ch["desc"].append(dsc[perm]); ch["last_query"].append(lq[perm]); ch["off"].append(ch["off"][-1] + len(xw))
-        per.append(dict(k=k, d=d, ur=ur))
-    cat = lambda xs, dt: np.ascontiguousarray(np.concatenate(xs).astype(dt))
-    fimg = np.arange(0, 2 * P, 2, dtype=np.int32)
-    hl = dict(fimg=fimg, off=np.array(last["off"], np.int32), Tcw=Tpred, dir=np.zeros(P, np.int32), xw=cat(last["xw"], np.float32), oct=cat(last["oct"], np.int32),
-              ang=cat(last["ang"], np.float32), desc=cat(last["desc"], np.uint8), obs=cat(last["obs"], np.uint8))
-    hc = dict(off=np.array(ch["off"], np.int32), xw=cat(ch["xw"], np.float32), normal=cat(ch["normal"], np.float32), max_dist=cat(ch["max_dist"], np.float32),
-              min_dist=cat(ch["min_dist"], np.float32), desc=cat(ch["desc"], np.uint8), last_query=cat(ch["last_query"], np.int32))
-    npnt = int(hc["off"][-1])
-    rc = 2 * P * 1400
-    z = lambda shape, dt: np.zeros(shape, dt)
-    o = dict(kps=z(rc, KP_DTYPE), desc=z((rc, 32), np.uint8), ur=z(rc, np.float32), dep=z(rc, np.float32), n=z(2 * P, np.int32), offsets=z(2 * P + 1, np.int32),
-             fm=z(rc, np.int32), nm1=z(P, np.int32), mt=z(npnt, np.int32), nm2=z(P, np.int32), pose=z((2, P, 7), np.float64), inl=z((2, P), np.int32),
-             eoff=z((2, P + 1), np.int32), efeat=z((2, rc), np.int32), outl=z((2, rc), np.uint8), c_in_view=z(npnt, np.uint8), c_px=z(npnt, np.float32),
-             c_py=z(npnt, np.float32), c_pxr=z(npnt, np.float32), c_level=z(npnt, np.int32), c_vc=z(npnt, np.float32), c_pose=z((P, 7), np.float32))
-    TH_LAST, TH_LOC = 15.0, 3.0
-    step = replay.TrackingStep(ex, cam, BF, B, TH_LAST, TH_LOC, 0.8, True)
-    step.submit(imgs, last=hl, pose=Tpred, chain=hc)
-    rows = step.collect(o)
-    assert rows == int(off[-1]) and (o["offsets"] == off).all()
-    logsf = np.float32(np.log(np.float32(1.2)))
-    cam5 = np.float32([FX, FY, CX, CY, BF])
-    checked = dict(released=0, skipped=0, in_view=0, local=0, both=0)
-    for p in range(P):
-        a, b = int(off[2 * p]), int(off[2 * p + 1])
-        k, d, ur = per[p]["k"], per[p]["d"], per[p]["ur"]
-        l0, l1, c0, c1 = int(hl["off"][p]), int(hl["off"][p + 1]), int(hc["off"][p]), int(hc["off"][p + 1])
-        xwL, obsL = hl["xw"][l0:l1], hl["obs"][l0:l1]
-        # 1. the motion-model search
-        fm0, nm0 = po.search_last(k, d, ur, BOUNDS, sf, CAM6, Tpred[p], 0, xwL, hl["oct"][l0:l1], hl["ang"][l0:l1], hl["desc"][l0:l1], obsL, TH_LAST, True)
-        assert nm0 == o["nm1"][p] and nm0 > 80
-        # 2. its PoseOptimization: one edge per matched feature, in feature order
-        feat = np.nonzero(fm0 >= 0)[0]
-        e0, e1 = int(o["eoff"][0][p]), int(o["eoff"][0][p + 1])
-        assert (o["efeat"][0][e0:e1] == feat).all()
-        obs3 = np.stack([k["x"][feat], k["y"][feat], ur[feat]], 1)
-        want1 = po.pose_optimization(Tpred[p], xwL[fm0[feat]], obs3, isg[k["octave"][feat]], cam5)
-        assert (o["outl"][0][e0:e1] == want1["outlier"]).all() and o["inl"][0][p] == want1["inliers"]
-        assert np.abs(o["pose"][0][p] - want1["pose"]).max() < 1e-4
-        # 3. outliers released; claims of the local-map search
-        fm1 = fm0.copy()
-        fm1[feat[want1["outlier"] != 0]] = -1
-        got_fm = o["fm"][a:b].copy()
-        got_fm[got_fm >= 0] -= l0
-        assert (got_fm == fm1).all()
-        checked["released"] += int((want1["outlier"] != 0).sum())
-        claimed = ((fm1 >= 0) & (obsL[np.maximum(fm1, 0)] != 0)).astype(np.uint8)
-        seen = np.zeros(l1 - l0, bool)
-        seen[fm0[feat]] = True
-        # 4. the pose the frame holds (Sophus::SE3f) and its matrices, from the DEVICE's first pose
-        posef, R, t, Ow = _se3f_from_pose(o["pose"][0][p])
-        assert (o["c_pose"][p].view(np.uint32) == posef.view(np.uint32)).all()
-        # 5. Frame::isInFrustum of the local map points, minus the ones the motion-model search already put into the frame
-        fr = po.is_in_frustum(R, t, Ow, BOUNDS, CAM6, 8, logsf, hc["xw"][c0:c1], hc["normal"][c0:c1], hc["max_dist"][c0:c1], hc["min_dist"][c0:c1], 0.5)
-        lq = hc["last_query"][c0:c1]
-        skip = (lq >= 0) & seen[np.maximum(lq, 0)]
-        vis = fr["in_view"].astype(bool) & ~skip
-        assert (o["c_in_view"][c0:c1].astype(bool) == vis).all()
-        for key, arr in (("proj_x", "c_px"), ("proj_y", "c_py"), ("proj_xr", "c_pxr"), ("view_cos", "c_vc")):
-            assert (o[arr][c0:c1][vis].view(np.uint32) == fr[key][vis].view(np.uint32)).all(), key
-        assert (o["c_level"][c0:c1][vis] == fr["level"][vis]).all()
-        checked["skipped"] += int(skip.sum()); checked["in_view"] += int(vis.sum())
-        # 6. SearchByProjection(F, local map points): the in-view ones, in list order, against the claims
-        vi = np.nonzero(vis)[0]
-        mt_v, nm2 = po.search_local(k, d, ur, BOUNDS, sf, fr["proj_x"][vi], fr["proj_y"][vi], fr["proj_xr"][vi], fr["level"][vi], fr["view_cos"][vi],
-                                    hc["desc"][c0:c1][vi], TH_LOC, 0.8, claimed=claimed, trackdepth=fr["depth"][vi])
-        want_mt = np.full(c1 - c0, -1, np.int32)
-        want_mt[vi] = mt_v
-        assert (o["mt"][c0:c1] == want_mt).all() and nm2 == o["nm2"][p] and nm2 > 100
-        checked["local"] += int(nm2)
-        # 7. PoseOptimization over every map point the frame holds: motion-model survivors + local-map matches (the latter win a feature)
-        holder = fm1.copy()
-        src2 = np.zeros(len(k), bool)
-        for q_ in np.nonzero(want_mt >= 0)[0]:
-            checked["both"] += int(holder[want_mt[q_]] >= 0)
-            holder[want_mt[q_]] = q_
-            src2[want_mt[q_]] = True
-        feat2 = np.nonzero(holder >= 0)[0]
-        e0, e1 = int(o["eoff"][1][p]), int(o["eoff"][1][p + 1])
-        assert (o["efeat"][1][e0:e1] == feat2).all()
-        xw2 = np.where(src2[feat2][:, None], hc["xw"][c0:c1][holder[feat2]], xwL[np.minimum(holder[feat2], len(xwL) - 1)])
-        obs3 = np.stack([k["x"][feat2], k["y"][feat2], ur[feat2]], 1)
-        want2 = po.pose_optimization(posef, xw2, obs3, isg[k["octave"][feat2]], cam5)
-        assert (o["outl"][1][e0:e1] == want2["outlier"]).all() and o["inl"][1][p] == want2["inliers"]
-        assert np.abs(o["pose"][1][p] - want2["pose"]).max() < 1e-4
+        st = np.nonzero(dep[a:b] > 0)[0]
+        frames.append(dict(k=kps[a:b], d=desc[a:b], z=dep[a:b], ur=uR[a:b], last=st[::2], other=st[1::2], rows=(a, b)))
+    step = replay.TrackingStep(ex, camera(FX, FY, CX, CY, BF, B, W, H), BF, B, 15.0, 3.0, 0.8, True)
+    _, _, nm0, nm2, checked = run_chained_flow(ex, step, imgs, off, frames, np.float32([FX, FY, CX, CY, BF, B]),
+                                               np.arange(0, 2 * P, 2, dtype=np.int32), 2 * P * 1400, 15.0, 3.0)
+    assert nm0.min() > 80 and nm2.min() > 100, (nm0, nm2)
     assert checked["released"] >= 3 and checked["skipped"] > 100 and checked["in_view"] > 400 and checked["local"] > 300, checked
     ex.close()

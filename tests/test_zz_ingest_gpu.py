@@ -14,9 +14,10 @@ import numpy as np
 import pytest
 import torch
 
+from _tracking import run_step, same_results
 from orb_slam3_detailed_comments_b200 import ORBextractor, camera, synth, replay
 from orb_slam3_detailed_comments_b200 import _native as N
-from orb_slam3_detailed_comments_b200._native import KP_DTYPE, OrbError
+from orb_slam3_detailed_comments_b200._native import OrbError
 from oracle import pyingest
 
 pytestmark = pytest.mark.gpu
@@ -80,30 +81,15 @@ def _queries(ex, grey, nimg, mono):
 
 
 def _run(ex, images, fmt, resize, mono, q):
-    hl, hc = q
-    nimg = len(images)
-    nf = nimg if mono else nimg // 2
     st = replay.TrackingStep(ex, camera(FX, FY, W / 2, H / 2, BF, B, W, H), BF, B, 15.0, 3.0, 0.8, True, monocular=mono,
                              image_format=fmt, resize=resize)
-    st.submit(images, last=hl, local=hc, pose=hl["Tcw"], local_world_pos=hc["xw"])
-    rc, nq = nimg * 1400, int(hc["off"][-1])
-    z = lambda shape, dt: np.zeros(shape, dt)
-    o = dict(kps=z(rc, KP_DTYPE), desc=z((rc, 32), np.uint8), ur=z(rc, f32), dep=z(rc, f32), n=z(nimg, np.int32), offsets=z(nimg + 1, np.int32),
-             fm=z(rc, np.int32), nm1=z(nf, np.int32), mt=z(nq, np.int32), nm2=z(nf, np.int32), pose=z((2, nf, 7), np.float64),
-             inl=z((2, nf), np.int32), eoff=z((2, nf + 1), np.int32), efeat=z((2, rc), np.int32), outl=z((2, rc), np.uint8))
-    rows = st.collect(o)
-    return rows, o
+    return run_step(st, images, *q)
 
 
-def _assert_same(a, b):
-    (ra, oa), (rb, ob) = a, b
-    assert ra == rb and ra > 0
-    assert (oa["n"] == ob["n"]).all() and (oa["offsets"] == ob["offsets"]).all()
-    assert (oa["kps"][:ra].view(np.uint8) == ob["kps"][:rb].view(np.uint8)).all() and (oa["desc"][:ra] == ob["desc"][:rb]).all()
-    assert (oa["ur"][:ra].view(np.uint32) == ob["ur"][:rb].view(np.uint32)).all() and (oa["dep"][:ra].view(np.uint32) == ob["dep"][:rb].view(np.uint32)).all()
-    for k in ("fm", "nm1", "mt", "nm2", "pose", "inl", "eoff"):
-        assert (oa[k] == ob[k]).all(), k
-    assert oa["nm1"].min() > 50 and oa["nm2"].min() > 50
+def _assert_same(got, want, mono):
+    same_results(got, want, stereo=not mono)
+    rows, o = got
+    assert rows > 0 and o["nm1"].min() > 50 and o["nm2"].min() > 50
 
 
 @pytest.fixture(scope="module")
@@ -123,7 +109,7 @@ def test_camera_step_equals_grey_step_on_oracle_images(handles, fmt, resized, mo
     q = _queries(handles["ref"], grey, len(grey), mono)
     want = _run(handles["ref"], grey, "gray", None, mono, q)
     got = _run(handles["step"], images, fmt, (W, H) if resized else None, mono, q)
-    _assert_same(got, want)
+    _assert_same(got, want, mono)
 
 
 @pytest.mark.parametrize("cn,rgb", [(1, False), (3, False), (3, True), (4, False), (4, True)])
@@ -200,7 +186,7 @@ def test_refusals_leave_the_handle_usable(handles):
     after = ex.download(2)
     assert all((x.view(np.uint8) == y.view(np.uint8)).all() for x, y in zip(after, before))
     q = _queries(handles["ref"], grey, 2, False)
-    _assert_same(_run(ex, grey, "gray", None, False, q), _run(handles["ref"], grey, "gray", None, False, q))
+    _assert_same(_run(ex, grey, "gray", None, False, q), _run(handles["ref"], grey, "gray", None, False, q), False)
 
 
 def test_grey_and_colour_steps_alternate_without_leaking(handles):
@@ -214,5 +200,5 @@ def test_grey_and_colour_steps_alternate_without_leaking(handles):
     want_b = _run(handles["ref"], oracle_b, "gray", None, False, qb)
     ex = handles["step"]
     for _ in range(2):
-        _assert_same(_run(ex, grey_a, "gray", None, False, qa), want_a)
-        _assert_same(_run(ex, colour_b, "rgb", (W, H), False, qb), want_b)
+        _assert_same(_run(ex, grey_a, "gray", None, False, qa), want_a, False)
+        _assert_same(_run(ex, colour_b, "rgb", (W, H), False, qb), want_b, False)

@@ -19,9 +19,8 @@ import pytest
 from oracle import pyoracle as po
 from orb_slam3_detailed_comments_b200 import (ORBextractor, ORBmatcher, PoseEdgesDevice, PoseOptimization, PoseOptimizationFrames, camera,
                                               replay, synth)
-from orb_slam3_detailed_comments_b200._native import KP_DTYPE
+from _tracking import chain_queries, check_chained_flow, step_outputs
 from test_poseopt_gpu import qR, quat
-from test_zz_chain_gpu import _se3f_from_pose
 from test_zz_many_features_gpu import cam_for, kitti, scene4k16k, step_queries   # noqa: F401  (kitti, scene4k16k: module fixtures)
 
 pytestmark = pytest.mark.gpu
@@ -425,19 +424,6 @@ def step16k(scene4k16k):
     e.close()
 
 
-def step_out(rc, nf, nq, chain_points=0):
-    z = lambda shape, dt: np.zeros(shape, dt)
-    o = dict(kps=z(rc, KP_DTYPE), desc=z((rc, 32), np.uint8), ur=z(rc, np.float32), dep=z(rc, np.float32), n=z(2 * nf, np.int32),
-             offsets=z(2 * nf + 1, np.int32), fm=z(rc, np.int32), nm1=z(nf, np.int32), mt=z(max(nq, 1), np.int32), nm2=z(nf, np.int32),
-             pose=z((2, nf, 7), np.float64), inl=z((2, nf), np.int32), eoff=z((2, nf + 1), np.int32), efeat=z((2, rc), np.int32),
-             outl=z((2, rc), np.uint8))
-    if chain_points:
-        np_ = chain_points
-        o.update(c_in_view=z(np_, np.uint8), c_px=z(np_, np.float32), c_py=z(np_, np.float32), c_pxr=z(np_, np.float32),
-                 c_level=z(np_, np.int32), c_vc=z(np_, np.float32), c_pose=z((nf, 7), np.float32))
-    return o
-
-
 def test_replay_step_with_pose_optimization_16k(scene4k16k, step16k):
     """orbr_submit with PoseOptimization after both searches on 16 000-feature frames: poses, inliers, edge tables and outlier flags equal
     the per-call path (each search, then PoseOptimizationFrames on its result arrays) and the oracle."""
@@ -457,7 +443,7 @@ def test_replay_step_with_pose_optimization_16k(scene4k16k, step16k):
     local_xw = hl["xw"]                                 # step_queries draws both query sets from the same points, in the same order
     per_call = [PoseOptimizationFrames(ex, hl["fimg"], hl["Tcw"], hl["xw"], cam5, feature_match=fm, total_rows=rows),
                 PoseOptimizationFrames(ex, hc["fimg"], hl["Tcw"], local_xw, cam5, query_offset=hc["off"], query_match=mt, total_rows=rows)]
-    o = step_out(2 * P * 16160, P, int(hc["off"][-1]))
+    o = step_outputs(2 * P, P, 2 * P * 16160, int(hc["off"][-1]))
     st = replay.TrackingStep(step16k, cam, bf, b, 15.0, 3.0, 0.8, True)
     st.submit(np.ascontiguousarray(S["imgs"]), last=hl, local=hc, pose=hl["Tcw"], local_world_pos=local_xw)
     assert st.collect(o) == rows and (o["offsets"] == off).all()
@@ -490,9 +476,9 @@ def test_chained_flow_16k(scene4k16k, step16k):
     pose rotated by 40 degrees with the camera 50 m from the world origin.  The handle's 16 160 rows size both edge walks' launches."""
     S = scene4k16k
     P, W, H = S["P"], S["w"], S["h"]
-    FX, FY, CX, CY, BF, B = S["cam6"]
+    BF, B = S["cam6"][4:]
     CAM6, BOUNDS = np.float32(S["cam6"]), np.float32([0, W, 0, H])
-    cam, cam5 = camera(*S["cam6"], W, H), np.float32(S["cam6"][:5])
+    cam = camera(*S["cam6"], W, H)
     rng = np.random.default_rng(83)
     ex, off, kps, desc, dep, uR = S["ex"], S["off"], S["kps"], S["desc"], S["dep"], S["uR"]
     sf, isg = ex.GetScaleFactors(), ex.GetInverseScaleSigmaSquares()
@@ -507,117 +493,24 @@ def test_chained_flow_16k(scene4k16k, step16k):
         qp = qmul(dq, q)
         Tpred[p] = np.concatenate([qp / np.linalg.norm(qp), qR(dq) @ t + rng.normal(0, 0.001, 3)]).astype(np.float32)
     Tpred[:, :4] /= np.linalg.norm(Tpred[:, :4], axis=1)[:, None]
-    last = dict(off=[0], xw=[], oct=[], ang=[], desc=[], obs=[])
-    ch = dict(off=[0], xw=[], normal=[], max_dist=[], min_dist=[], desc=[], last_query=[])
+    frames = []
     for p in range(P):
         a, b = int(off[2 * p]), int(off[2 * p + 1])
-        k, d, z = kps[a:b], desc[a:b], dep[a:b]
-        R, t = Ttrue[p]
-        st = np.nonzero(z > 0)[0]
-        selL, selB = st[::2], st[1::2]
-        cpts = lambda s: np.stack([(k["x"][s] - CX) * z[s] / FX, (k["y"][s] - CY) * z[s] / FY, z[s]], 1)
-        world = lambda Xc: ((Xc - t) @ R).astype(np.float32)
-        XcL = cpts(selL)
-        gross = rng.random(len(selL)) < 0.06          # 12 px to the side: inside the search window, then thrown out by PoseOptimization
-        XcL[gross, 0] += 12 * z[selL][gross] / FX
-        xwL = world(XcL)
-        Oc = (-R.T @ t).astype(np.float32)
-        last["xw"].append(xwL); last["oct"].append(k["octave"][selL].astype(np.int32)); last["ang"].append(k["angle"][selL].astype(np.float32))
-        last["desc"].append(d[selL]); last["obs"].append((rng.random(len(selL)) < 0.9).astype(np.uint8)); last["off"].append(last["off"][-1] + len(selL))
-        nC = 1000
-        xwB = world(cpts(selB))
-        xwC = ((np.stack([rng.uniform(-60, 60, nC), rng.uniform(-40, 40, nC), rng.uniform(-10, 80, nC)], 1) - t) @ R).astype(np.float32)
-        xw = np.concatenate([xwL, xwB, xwC])
-        dsc = np.concatenate([d[selL], d[selB], rng.integers(0, 256, (nC, 32), dtype=np.uint8)])
-        lq = np.concatenate([np.arange(len(selL)), np.full(len(selB) + nC, -1)]).astype(np.int32)
-        octs = np.concatenate([k["octave"][selL], k["octave"][selB], rng.integers(0, 8, nC)])
-        dist = np.linalg.norm(xw - Oc, axis=1).astype(np.float32)
-        maxd = (dist * sf[octs] * rng.uniform(0.75, 1.3, len(xw))).astype(np.float32)
-        nrm = (xw - Oc) / np.maximum(dist[:, None], 1e-6) + rng.normal(0, 0.35, xw.shape)
-        nrm = (nrm / np.linalg.norm(nrm, axis=1)[:, None]).astype(np.float32)
-        perm = rng.permutation(len(xw))
-        ch["xw"].append(xw[perm]); ch["normal"].append(nrm[perm]); ch["max_dist"].append(maxd[perm])
-        ch["min_dist"].append((maxd / sf[7]).astype(np.float32)[perm]); ch["desc"].append(dsc[perm]); ch["last_query"].append(lq[perm])
-        ch["off"].append(ch["off"][-1] + len(xw))
-    cat = lambda xs, dt: np.ascontiguousarray(np.concatenate(xs).astype(dt))
-    hl = dict(fimg=np.arange(0, 2 * P, 2, dtype=np.int32), off=np.array(last["off"], np.int32), Tcw=Tpred, dir=np.zeros(P, np.int32),
-              xw=cat(last["xw"], np.float32), oct=cat(last["oct"], np.int32), ang=cat(last["ang"], np.float32), desc=cat(last["desc"], np.uint8),
-              obs=cat(last["obs"], np.uint8))
-    hc = dict(off=np.array(ch["off"], np.int32), xw=cat(ch["xw"], np.float32), normal=cat(ch["normal"], np.float32),
-              max_dist=cat(ch["max_dist"], np.float32), min_dist=cat(ch["min_dist"], np.float32), desc=cat(ch["desc"], np.uint8),
-              last_query=cat(ch["last_query"], np.int32))
+        st = np.nonzero(dep[a:b] > 0)[0]
+        frames.append(dict(k=kps[a:b], d=desc[a:b], z=dep[a:b], ur=uR[a:b], last=st[::2], other=st[1::2], rows=(a, b)))
+    # the map in world coordinates: gross errors 12 px to the side, 1 000 points around each camera, mostly out of view
+    hl, hc = chain_queries(frames, rng, sf, CAM6, Tpred, np.arange(0, 2 * P, 2, dtype=np.int32), gross_px=12, n_far=1000,
+                           far_box=((-60, 60), (-40, 40), (-10, 80)), world=Ttrue)
     npnt = int(hc["off"][-1])
-    o = step_out(2 * P * 16160, P, npnt, chain_points=npnt)
-    TH_LAST, TH_LOC = 15.0, 3.0
-    step = replay.TrackingStep(step16k, cam, BF, B, TH_LAST, TH_LOC, 0.8, True)
+    o = step_outputs(2 * P, P, 2 * P * 16160, npnt, chain_points=npnt)
+    step = replay.TrackingStep(step16k, cam, BF, B, 15.0, 3.0, 0.8, True)
     step.submit(np.ascontiguousarray(S["imgs"]), last=hl, pose=Tpred, chain=hc)
     rows = step.collect(o)
     assert rows == int(off[-1]) and (o["offsets"] == off).all()
     assert (o["kps"][:rows].view(np.uint8) == kps.view(np.uint8)).all() and (o["ur"][:rows].view(np.uint32) == uR.view(np.uint32)).all()
-    logsf = np.float32(np.log(np.float32(1.2)))
-    checked = dict(released=0, skipped=0, in_view=0, local=0, both=0)
-    for p in range(P):
-        a, b = int(off[2 * p]), int(off[2 * p + 1])
-        k, d, ur = kps[a:b], desc[a:b], uR[a:b]
-        l0, l1, c0, c1 = int(hl["off"][p]), int(hl["off"][p + 1]), int(hc["off"][p]), int(hc["off"][p + 1])
-        xwL, obsL = hl["xw"][l0:l1], hl["obs"][l0:l1]
-        # 1. the motion-model search
-        fm0, nm0 = po.search_last(k, d, ur, BOUNDS, sf, CAM6, Tpred[p], 0, xwL, hl["oct"][l0:l1], hl["ang"][l0:l1], hl["desc"][l0:l1], obsL, TH_LAST, True)
-        assert nm0 == o["nm1"][p] and nm0 > 150, (p, nm0, o["nm1"][p])     # the scene's stereo rows are few (~600 per frame)
-        # 2. its PoseOptimization: one edge per matched feature, in feature order
-        feat = np.nonzero(fm0 >= 0)[0]
-        e0, e1 = int(o["eoff"][0][p]), int(o["eoff"][0][p + 1])
-        assert (o["efeat"][0][e0:e1] == feat).all()
-        obs3 = np.stack([k["x"][feat], k["y"][feat], ur[feat]], 1)
-        want1 = po.pose_optimization(Tpred[p], xwL[fm0[feat]], obs3, isg[k["octave"][feat]], cam5)
-        assert (o["outl"][0][e0:e1] == want1["outlier"]).all() and o["inl"][0][p] == want1["inliers"]
-        assert np.abs(o["pose"][0][p] - want1["pose"]).max() < TOL
-        # 3. outliers released; claims of the local-map search
-        fm1 = fm0.copy()
-        fm1[feat[want1["outlier"] != 0]] = -1
-        got_fm = o["fm"][a:b].copy()
-        got_fm[got_fm >= 0] -= l0
-        assert (got_fm == fm1).all()
-        checked["released"] += int((want1["outlier"] != 0).sum())
-        claimed = ((fm1 >= 0) & (obsL[np.maximum(fm1, 0)] != 0)).astype(np.uint8)
-        seen = np.zeros(l1 - l0, bool)
-        seen[fm0[feat]] = True
-        # 4. the pose the frame holds (Sophus::SE3f) and its matrices, from the device's first pose
-        posef, R, t, Ow = _se3f_from_pose(o["pose"][0][p])
-        assert (o["c_pose"][p].view(np.uint32) == posef.view(np.uint32)).all()
-        # 5. Frame::isInFrustum of the local map points, minus the ones the motion-model search already put into the frame
-        fr = po.is_in_frustum(R, t, Ow, BOUNDS, CAM6, 8, logsf, hc["xw"][c0:c1], hc["normal"][c0:c1], hc["max_dist"][c0:c1], hc["min_dist"][c0:c1], 0.5)
-        lq = hc["last_query"][c0:c1]
-        skip = (lq >= 0) & seen[np.maximum(lq, 0)]
-        vis = fr["in_view"].astype(bool) & ~skip
-        assert (o["c_in_view"][c0:c1].astype(bool) == vis).all()
-        for key, arr in (("proj_x", "c_px"), ("proj_y", "c_py"), ("proj_xr", "c_pxr"), ("view_cos", "c_vc")):
-            assert (o[arr][c0:c1][vis].view(np.uint32) == fr[key][vis].view(np.uint32)).all(), key
-        assert (o["c_level"][c0:c1][vis] == fr["level"][vis]).all()
-        checked["skipped"] += int(skip.sum()); checked["in_view"] += int(vis.sum())
-        # 6. SearchByProjection(F, local map points): the in-view ones, in list order, against the claims
-        vi = np.nonzero(vis)[0]
-        mt_v, nm2 = po.search_local(k, d, ur, BOUNDS, sf, fr["proj_x"][vi], fr["proj_y"][vi], fr["proj_xr"][vi], fr["level"][vi], fr["view_cos"][vi],
-                                    hc["desc"][c0:c1][vi], TH_LOC, 0.8, claimed=claimed, trackdepth=fr["depth"][vi])
-        want_mt = np.full(c1 - c0, -1, np.int32)
-        want_mt[vi] = mt_v
-        assert (o["mt"][c0:c1] == want_mt).all() and nm2 == o["nm2"][p] and nm2 > 100, (p, nm2)
-        checked["local"] += int(nm2)
-        # 7. PoseOptimization over every map point the frame holds: motion-model survivors + local-map matches (the latter win a feature)
-        holder = fm1.copy()
-        src2 = np.zeros(len(k), bool)
-        for q_ in np.nonzero(want_mt >= 0)[0]:
-            checked["both"] += int(holder[want_mt[q_]] >= 0)
-            holder[want_mt[q_]] = q_
-            src2[want_mt[q_]] = True
-        feat2 = np.nonzero(holder >= 0)[0]
-        e0, e1 = int(o["eoff"][1][p]), int(o["eoff"][1][p + 1])
-        assert (o["efeat"][1][e0:e1] == feat2).all()
-        xw2 = np.where(src2[feat2][:, None], hc["xw"][c0:c1][holder[feat2]], xwL[np.minimum(holder[feat2], len(xwL) - 1)])
-        obs3 = np.stack([k["x"][feat2], k["y"][feat2], ur[feat2]], 1)
-        want2 = po.pose_optimization(posef, xw2, obs3, isg[k["octave"][feat2]], cam5)
-        assert (o["outl"][1][e0:e1] == want2["outlier"]).all() and o["inl"][1][p] == want2["inliers"]
-        assert np.abs(o["pose"][1][p] - want2["pose"]).max() < TOL
-        # the optimised pose is the true one to within the noise of 16 000 matches
-        assert np.abs(o["pose"][1][p][4:] - Ttrue[p][1]).max() < 0.05, (p, o["pose"][1][p][4:], Ttrue[p][1])
+    nm0, nm2, checked = check_chained_flow(o, hl, hc, frames, CAM6, BOUNDS, sf, isg, 15.0, 3.0)
+    assert nm0.min() > 150 and nm2.min() > 100, (nm0, nm2)      # the scene's stereo rows are few (~600 per frame)
     assert checked["released"] >= 3 and checked["skipped"] > 300 and checked["in_view"] > 400 and checked["local"] > 200, checked
+    # the optimised pose is the true one to within the noise of 16 000 matches
+    for p in range(P):
+        assert np.abs(o["pose"][1][p][4:] - Ttrue[p][1]).max() < 0.05, (p, o["pose"][1][p][4:], Ttrue[p][1])

@@ -6,8 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from orb_slam3_detailed_comments_b200 import ORBextractor, ORBmatcher, camera, synth, PoseOptimizationFrames, replay
-from orb_slam3_detailed_comments_b200._native import KP_DTYPE
+from _tracking import check_against_per_call, step_outputs
+from orb_slam3_detailed_comments_b200 import ORBextractor, camera, synth, replay
 from oracle import pyoracle as po
 
 pytestmark = pytest.mark.gpu
@@ -46,13 +46,6 @@ def _queries(ex, imgs, P, rng):
     return hl, hc
 
 
-def _outputs(P, rc, nloc):
-    z = lambda shape, dt: np.zeros(shape, dt)
-    return dict(kps=z(rc, KP_DTYPE), desc=z((rc, 32), np.uint8), ur=z(rc, np.float32), dep=z(rc, np.float32), n=z(2 * P, np.int32),
-                offsets=z(2 * P + 1, np.int32), fm=z(rc, np.int32), nm1=z(P, np.int32), mt=z(max(nloc, 1), np.int32), nm2=z(P, np.int32),
-                pose=z((2, P, 7), np.float64), inl=z((2, P), np.int32), eoff=z((2, P + 1), np.int32), efeat=z((2, rc), np.int32), outl=z((2, rc), np.uint8))
-
-
 @pytest.mark.parametrize("with_po", [False, True])
 def test_replay_step_equals_blocking_calls(with_po):
     P = 2
@@ -61,11 +54,9 @@ def test_replay_step_equals_blocking_calls(with_po):
     batches = [np.stack([im for p in range(P) for im in synth.stereo_pair(W, H, seed=900 + 10 * s + p)[:2]]) for s in range(3)]
     ref = ORBextractor(NF, 1.2, 8, 20, 7, max_width=W, max_height=H, max_batch=2 * P)
     exs = [ORBextractor(NF, 1.2, 8, 20, 7, max_width=W, max_height=H, max_batch=2 * P) for _ in range(2)]
-    m_last, m_loc = ORBmatcher(0.9, True), ORBmatcher(0.8, True)
     qs = [_queries(ref, b, P, rng) for b in batches]
-    rc = 2 * P * 1400
     steps = [replay.TrackingStep(e, cam, BF, B, 15.0, 3.0, 0.8, True) for e in exs]
-    outs = [_outputs(P, rc, max(int(q[1]["off"][-1]) for q in qs)) for _ in exs]
+    outs = [step_outputs(2 * P, P, 2 * P * 1400, max(int(q[1]["off"][-1]) for q in qs)) for _ in exs]
 
     def submit(i):
         hl, hc = qs[i]
@@ -90,22 +81,8 @@ def test_replay_step_equals_blocking_calls(with_po):
             left[int(off[2 * p]):int(off[2 * p + 1])] = True
         assert (o["kps"][:rows].view(np.uint8) == kps.view(np.uint8)).all() and (o["desc"][:rows] == desc).all()
         assert (o["ur"][:rows].view(np.uint32)[left] == uR.view(np.uint32)[left]).all() and (o["dep"][:rows].view(np.uint32)[left] == dep.view(np.uint32)[left]).all()
-        fm, nm1 = m_last.SearchByProjectionLastFrame(ref, cam, hl["fimg"], hl["off"], hl["Tcw"], hl["dir"], hl["xw"], hl["oct"], hl["ang"], hl["desc"], hl["obs"], 15.0, rows)
-        assert (o["fm"][:rows] == fm).all() and (o["nm1"] == nm1).all() and nm1.min() > 50
-        mt, nm2 = m_loc.SearchByProjection(ref, cam, hc["fimg"], hc["off"], hc["px"], hc["py"], hc["pxr"], hc["lvl"], hc["vc"], hc["desc"], th=3.0)
-        nq = int(hc["off"][-1])
-        assert (o["mt"][:nq] == mt).all() and (o["nm2"] == nm2).all() and nm2.min() > 200
-        if with_po:
-            cam5 = [FX, FY, CX, CY, BF]
-            pose1, outl1, inl1 = PoseOptimizationFrames(ref, hl["fimg"], hl["Tcw"], hl["xw"], cam5, feature_match=fm, total_rows=rows)
-            pose2, outl2, inl2 = PoseOptimizationFrames(ref, hc["fimg"], hl["Tcw"], hc["xw"], cam5, query_offset=hc["off"], query_match=mt, total_rows=rows)
-            for k, (pose, outl, inl) in enumerate([(pose1, outl1, inl1), (pose2, outl2, inl2)]):
-                assert (o["pose"][k] == pose).all() and (o["inl"][k] == inl).all() and inl.min() > 30
-                got = np.zeros(rows, np.uint8)
-                for p in range(P):
-                    e0, e1 = int(o["eoff"][k][p]), int(o["eoff"][k][p + 1])
-                    got[int(off[2 * p]) + o["efeat"][k][e0:e1]] = o["outl"][k][e0:e1]
-                assert (got == outl).all()
+        nm1, nm2, inl = check_against_per_call(o, rows, ref, cam, hl, hc, 15.0, 3.0, [FX, FY, CX, CY, BF], with_po)
+        assert nm1.min() > 50 and nm2.min() > 200 and (inl is None or inl.min() > 30)
     # first frame against the CPU oracle directly (extraction bytes)
     eo = po.OracleExtractor(NF, 1.2, 8, 20, 7)
     _, rk, rd = eo(batches[2][0])

@@ -8,14 +8,16 @@ conversion, k_stereo_rgbd) and the RGB-D replay step (orbr_step::depth_maps).
   answer differs from the oracle's with mvuRight = -1: the gates are live;
 - the chained flow in RGB-D mode matches the oracle stage by stage;
 - a CUDA-graph replay of the device-resident step equals the eager calls;
-- every refusal leaves the handle usable; stereo, monocular and RGB-D steps alternating on one handle leak no state;
+- every refusal leaves the handle usable; stereo, monocular and RGB-D steps alternating on one handle, with and without PoseOptimization,
+  leak no state;
 - orbx_pack_keyframe_device carries the depth-derived uright of an RGB-D frame."""
 import numpy as np
 import pytest
 import torch
 
-from orb_slam3_detailed_comments_b200 import ORBextractor, ORBmatcher, camera, synth, PoseOptimizationFrames, replay
-from orb_slam3_detailed_comments_b200._native import KP_DTYPE, OrbError
+from _tracking import check_against_per_call, run_chained_flow, run_step, same_results, step_outputs
+from orb_slam3_detailed_comments_b200 import ORBextractor, ORBmatcher, camera, synth, replay
+from orb_slam3_detailed_comments_b200._native import OrbError
 from oracle import pyingest
 from oracle import pyoracle as po
 from oracle import pyrgbd
@@ -98,13 +100,6 @@ def _per_call(ex, imgs, maps, bf):
     return n, off, kps, desc, uR.copy(), dep.copy()
 
 
-def _outputs(P, rc, nloc):
-    z = lambda shape, dt: np.zeros(shape, dt)
-    return dict(kps=z(rc, KP_DTYPE), desc=z((rc, 32), np.uint8), ur=z(rc, f32), dep=z(rc, f32), n=z(P, np.int32), offsets=z(P + 1, np.int32),
-                fm=z(rc, np.int32), nm1=z(P, np.int32), mt=z(max(nloc, 1), np.int32), nm2=z(P, np.int32), pose=z((2, P, 7), np.float64),
-                inl=z((2, P), np.int32), eoff=z((2, P + 1), np.int32), efeat=z((2, rc), np.int32), outl=z((2, rc), np.uint8))
-
-
 def _bits(a, b):
     return a.shape == b.shape and (np.ascontiguousarray(a).view(np.uint32) == np.ascontiguousarray(b).view(np.uint32)).all()
 
@@ -148,7 +143,6 @@ def test_rgbd_step_equals_blocking_calls_and_the_oracle(geom, direction, rgb):
     batches = [_frames(W, H, BF, [2200 + 10 * s + p for p in range(P)], rgb) for s in range(3)]
     ref = _mk(W, H, NF, P)
     exs = [_mk(W, H, NF, P) for _ in range(2)]
-    m_last, m_loc = ORBmatcher(0.9, True), ORBmatcher(0.8, True)
     qs = []
     for imgs, maps in batches:
         n, off, kps, desc, uR, dep = _per_call(ref, _grey(imgs), maps, BF)
@@ -156,7 +150,7 @@ def test_rgbd_step_equals_blocking_calls_and_the_oracle(geom, direction, rgb):
     rc = P * ref.max_features_per_image()
     fmt = "rgb" if rgb else "gray"
     steps = [replay.TrackingStep(e, cam, BF, BF / FX, TH_LAST, TH_LOC, 0.8, True, image_format=fmt, rgbd=True, depth_factor=FACTOR) for e in exs]
-    outs = [_outputs(P, rc, max(int(q[1]["off"][-1]) for q in qs)) for _ in exs]
+    outs = [step_outputs(P, P, rc, max(int(q[1]["off"][-1]) for q in qs)) for _ in exs]
 
     def submit(i):
         hl, hc = qs[i]
@@ -176,16 +170,8 @@ def test_rgbd_step_equals_blocking_calls_and_the_oracle(geom, direction, rgb):
         assert rows == int(off[-1]) and (o["n"] == n).all() and (o["offsets"] == off).all() and n.min() > 0.8 * NF
         assert (o["kps"][:rows].view(np.uint8) == kps.view(np.uint8)).all() and (o["desc"][:rows] == desc).all()
         assert _bits(o["ur"][:rows], uR) and _bits(o["dep"][:rows], dep) and (dep > 0).sum() > 0.8 * rows
-        fm, nm1 = m_last.SearchByProjectionLastFrame(ref, cam, hl["fimg"], hl["off"], hl["Tcw"], hl["dir"], hl["xw"], hl["oct"], hl["ang"], hl["desc"],
-                                                     hl["obs"], TH_LAST, rows)
-        assert (o["fm"][:rows] == fm).all() and (o["nm1"] == nm1).all() and nm1.min() > 50
-        mt, nm2 = m_loc.SearchByProjection(ref, cam, hc["fimg"], hc["off"], hc["px"], hc["py"], hc["pxr"], hc["lvl"], hc["vc"], hc["desc"], th=TH_LOC)
-        nq = int(hc["off"][-1])
-        assert (o["mt"][:nq] == mt).all() and (o["nm2"] == nm2).all() and nm2.min() > 100
-        pose1, outl1, inl1 = PoseOptimizationFrames(ref, hl["fimg"], hl["Tcw"], hl["xw"], cam5, feature_match=fm, total_rows=rows)
-        pose2, outl2, inl2 = PoseOptimizationFrames(ref, hc["fimg"], hl["Tcw"], hc["xw"], cam5, query_offset=hc["off"], query_match=mt, total_rows=rows)
-        for k, (pose, inl) in enumerate([(pose1, inl1), (pose2, inl2)]):
-            assert (o["pose"][k] == pose).all() and (o["inl"][k] == inl).all() and inl.min() > 30
+        nm1, nm2, inl = check_against_per_call(o, rows, ref, cam, hl, hc, TH_LAST, TH_LOC, cam5, True)
+        assert nm1.min() > 50 and nm2.min() > 100 and inl.min() > 30
     # the first frame of the last batch against the CPU oracle, fed the same depth-derived mvuRight
     o, off = outs[0], outs[0]["offsets"]          # batch 2 ran on handle 0
     hl, hc = qs[2]
@@ -232,123 +218,26 @@ def test_rgbd_step_equals_blocking_calls_and_the_oracle(geom, direction, rgb):
 
 # ---------------------------------------------------------------------------------------------------------------------------
 def test_rgbd_chained_flow_matches_the_oracle_stage_by_stage():
-    from test_zz_mono_step_gpu import _se3f_from_pose
-    g = GEOM["tum_640x480"]
-    W, H, NF, FX, FY, CX, CY, BF = g
+    W, H, NF, FX, FY, CX, CY, BF = GEOM["tum_640x480"]
     P = 2
-    rng = np.random.default_rng(5)
-    cam = camera(FX, FY, CX, CY, BF, BF / FX, W, H)
     imgs, maps = _frames(W, H, BF, [2400 + p for p in range(P)])
     ex = _mk(W, H, NF, P)
     _, off, kps, desc, uR, dep = _per_call(ex, imgs, maps, BF)
-    sf = ex.GetScaleFactors()
-    isg = ex.GetInverseScaleSigmaSquares()
-    bounds = f32([0, W, 0, H])
-    cam6 = f32([FX, FY, CX, CY, BF, BF / FX])
-    cam5 = f32([FX, FY, CX, CY, BF])
-    Tpred = np.tile(np.array([0.0005, -0.0008, 0.0003, 1, 0.004, -0.003, 0.002], f32), (P, 1))
-    Tpred[:, :4] /= np.linalg.norm(Tpred[:, :4], axis=1)[:, None]
-    last = dict(off=[0], xw=[], oct=[], ang=[], desc=[], obs=[])
-    ch = dict(off=[0], xw=[], normal=[], max_dist=[], min_dist=[], desc=[], last_query=[])
-    per = []
-    for p in range(P):
+    frames = []
+    for p in range(P):              # every feature at its depth-map depth (3 m in the holes); mvuRight from the depth map
         a, b = int(off[p]), int(off[p + 1])
-        k, d = kps[a:b], desc[a:b]
-        z = np.where(dep[a:b] > 0, dep[a:b], f32(3.0)).astype(f32)
-        allf = np.arange(len(k))
-        selL, selB = allf[::2], allf[1::2]
-        pts = lambda s: np.stack([(k["x"][s] - f32(CX)) * z[s] / f32(FX), (k["y"][s] - f32(CY)) * z[s] / f32(FY), z[s]], 1).astype(f32)
-        xwL = pts(selL)
-        gross = rng.random(len(selL)) < 0.06
-        xwL[gross, 0] += (f32(8.0) * xwL[gross, 2] / f32(FX)).astype(f32)
-        last["xw"].append(xwL); last["oct"].append(k["octave"][selL].astype(np.int32)); last["ang"].append(k["angle"][selL].astype(f32))
-        last["desc"].append(d[selL]); last["obs"].append((rng.random(len(selL)) < 0.9).astype(np.uint8)); last["off"].append(last["off"][-1] + len(selL))
-        nC = 200
-        xwB = pts(selB)
-        xwC = np.stack([rng.uniform(-30, 30, nC), rng.uniform(-20, 20, nC), rng.uniform(-10, 40, nC)], 1).astype(f32)
-        xw = np.concatenate([xwL, xwB, xwC])
-        dsc = np.concatenate([d[selL], d[selB], rng.integers(0, 256, (nC, 32), dtype=np.uint8)])
-        lq = np.concatenate([np.arange(len(selL)), np.full(len(selB) + nC, -1)]).astype(np.int32)
-        octs = np.concatenate([k["octave"][selL], k["octave"][selB], rng.integers(0, 8, nC)])
-        dist = np.linalg.norm(xw, axis=1).astype(f32)
-        maxd = (dist * sf[octs] * rng.uniform(0.75, 1.3, len(xw))).astype(f32)
-        nrm = xw / np.maximum(dist[:, None], 1e-6) + rng.normal(0, 0.35, xw.shape)
-        nrm = (nrm / np.linalg.norm(nrm, axis=1)[:, None]).astype(f32)
-        perm = rng.permutation(len(xw))
-        ch["xw"].append(xw[perm]); ch["normal"].append(nrm[perm]); ch["max_dist"].append(maxd[perm]); ch["min_dist"].append((maxd / sf[7]).astype(f32)[perm])
-        ch["desc"].append(dsc[perm]); ch["last_query"].append(lq[perm]); ch["off"].append(ch["off"][-1] + len(xw))
-        per.append(dict(k=k, d=d, ur=pyrgbd.stereo_from_rgbd(k, maps[p], FACTOR, BF)[0]))
-    cat = lambda xs, dt: np.ascontiguousarray(np.concatenate(xs).astype(dt))
-    hl = dict(fimg=np.arange(P, dtype=np.int32), off=np.array(last["off"], np.int32), Tcw=Tpred, dir=np.zeros(P, np.int32), xw=cat(last["xw"], f32),
-              oct=cat(last["oct"], np.int32), ang=cat(last["ang"], f32), desc=cat(last["desc"], np.uint8), obs=cat(last["obs"], np.uint8))
-    hc = dict(off=np.array(ch["off"], np.int32), xw=cat(ch["xw"], f32), normal=cat(ch["normal"], f32), max_dist=cat(ch["max_dist"], f32),
-              min_dist=cat(ch["min_dist"], f32), desc=cat(ch["desc"], np.uint8), last_query=cat(ch["last_query"], np.int32))
-    npnt = int(hc["off"][-1])
-    o = _outputs(P, P * ex.max_features_per_image(), npnt)
-    z_ = lambda shape, dt: np.zeros(shape, dt)
-    o.update(c_in_view=z_(npnt, np.uint8), c_px=z_(npnt, f32), c_py=z_(npnt, f32), c_pxr=z_(npnt, f32), c_level=z_(npnt, np.int32),
-             c_vc=z_(npnt, f32), c_pose=z_((P, 7), f32))
-    step = replay.TrackingStep(ex, cam, BF, BF / FX, TH_LAST, TH_LOC, 0.8, True, rgbd=True, depth_factor=FACTOR)
-    step.submit(imgs, last=hl, pose=Tpred, chain=hc, depth=maps)
-    rows = step.collect(o)
-    assert rows == int(off[-1]) and (o["offsets"] == off).all() and _bits(o["ur"][:rows], uR)
-    logsf = f32(np.log(f32(1.2)))
-    checked = dict(released=0, skipped=0, in_view=0, local=0, stereo=0)
-    for p in range(P):
-        a, b = int(off[p]), int(off[p + 1])
-        k, d, ur = per[p]["k"], per[p]["d"], per[p]["ur"]
-        l0, l1, c0, c1 = int(hl["off"][p]), int(hl["off"][p + 1]), int(hc["off"][p]), int(hc["off"][p + 1])
-        xwL, obsL = hl["xw"][l0:l1], hl["obs"][l0:l1]
-        fm0, nm0 = po.search_last(k, d, ur, bounds, sf, cam6, Tpred[p], 0, xwL, hl["oct"][l0:l1], hl["ang"][l0:l1], hl["desc"][l0:l1], obsL, TH_LAST, True)
-        assert nm0 == o["nm1"][p] and nm0 > 80
-        feat = np.nonzero(fm0 >= 0)[0]
-        e0, e1 = int(o["eoff"][0][p]), int(o["eoff"][0][p + 1])
-        assert (o["efeat"][0][e0:e1] == feat).all()
-        obs3 = np.stack([k["x"][feat], k["y"][feat], ur[feat]], 1)
-        checked["stereo"] += int((ur[feat] > 0).sum())
-        want1 = po.pose_optimization(Tpred[p], xwL[fm0[feat]], obs3, isg[k["octave"][feat]], cam5)
-        assert (o["outl"][0][e0:e1] == want1["outlier"]).all() and o["inl"][0][p] == want1["inliers"]
-        assert np.abs(o["pose"][0][p] - want1["pose"]).max() < 1e-4
-        fm1 = fm0.copy()
-        fm1[feat[want1["outlier"] != 0]] = -1
-        got_fm = o["fm"][a:b].copy()
-        got_fm[got_fm >= 0] -= l0
-        assert (got_fm == fm1).all()
-        checked["released"] += int((want1["outlier"] != 0).sum())
-        claimed = ((fm1 >= 0) & (obsL[np.maximum(fm1, 0)] != 0)).astype(np.uint8)
-        seen = np.zeros(l1 - l0, bool)
-        seen[fm0[feat]] = True
-        posef, R, t, Ow = _se3f_from_pose(o["pose"][0][p])
-        assert (o["c_pose"][p].view(np.uint32) == posef.view(np.uint32)).all()
-        fr = po.is_in_frustum(R, t, Ow, bounds, cam6, 8, logsf, hc["xw"][c0:c1], hc["normal"][c0:c1], hc["max_dist"][c0:c1], hc["min_dist"][c0:c1], 0.5)
-        lq = hc["last_query"][c0:c1]
-        skip = (lq >= 0) & seen[np.maximum(lq, 0)]
-        vis = fr["in_view"].astype(bool) & ~skip
-        assert (o["c_in_view"][c0:c1].astype(bool) == vis).all()
-        for key, arr in (("proj_x", "c_px"), ("proj_y", "c_py"), ("proj_xr", "c_pxr"), ("view_cos", "c_vc")):
-            assert (o[arr][c0:c1][vis].view(np.uint32) == fr[key][vis].view(np.uint32)).all(), key
-        checked["skipped"] += int(skip.sum()); checked["in_view"] += int(vis.sum())
-        vi = np.nonzero(vis)[0]
-        mt_v, nm2 = po.search_local(k, d, ur, bounds, sf, fr["proj_x"][vi], fr["proj_y"][vi], fr["proj_xr"][vi], fr["level"][vi], fr["view_cos"][vi],
-                                    hc["desc"][c0:c1][vi], TH_LOC, 0.8, claimed=claimed, trackdepth=fr["depth"][vi])
-        want_mt = np.full(c1 - c0, -1, np.int32)
-        want_mt[vi] = mt_v
-        assert (o["mt"][c0:c1] == want_mt).all() and nm2 == o["nm2"][p] and nm2 > 100
-        checked["local"] += int(nm2)
-        holder = fm1.copy()
-        src2 = np.zeros(len(k), bool)
-        for q_ in np.nonzero(want_mt >= 0)[0]:
-            holder[want_mt[q_]] = q_
-            src2[want_mt[q_]] = True
-        feat2 = np.nonzero(holder >= 0)[0]
-        e0, e1 = int(o["eoff"][1][p]), int(o["eoff"][1][p + 1])
-        assert (o["efeat"][1][e0:e1] == feat2).all()
-        xw2 = np.where(src2[feat2][:, None], hc["xw"][c0:c1][holder[feat2]], xwL[np.minimum(holder[feat2], len(xwL) - 1)])
-        obs3 = np.stack([k["x"][feat2], k["y"][feat2], ur[feat2]], 1)
-        want2 = po.pose_optimization(posef, xw2, obs3, isg[k["octave"][feat2]], cam5)
-        assert (o["outl"][1][e0:e1] == want2["outlier"]).all() and o["inl"][1][p] == want2["inliers"]
-        assert np.abs(o["pose"][1][p] - want2["pose"]).max() < 1e-4
-    assert checked["released"] >= 3 and checked["skipped"] > 100 and checked["in_view"] > 400 and checked["local"] > 200 and checked["stereo"] > 100, checked
+        k = kps[a:b]
+        frames.append(dict(k=k, d=desc[a:b], z=np.where(dep[a:b] > 0, dep[a:b], f32(3.0)).astype(f32),
+                           ur=pyrgbd.stereo_from_rgbd(k, maps[p], FACTOR, BF)[0], last=np.arange(0, b - a, 2), other=np.arange(1, b - a, 2),
+                           rows=(a, b)))
+    step = replay.TrackingStep(ex, camera(FX, FY, CX, CY, BF, BF / FX, W, H), BF, BF / FX, TH_LAST, TH_LOC, 0.8, True, rgbd=True,
+                               depth_factor=FACTOR)
+    rows, o, nm0, nm2, checked = run_chained_flow(ex, step, imgs, off, frames, f32([FX, FY, CX, CY, BF, BF / FX]), np.arange(P, dtype=np.int32),
+                                                  P * ex.max_features_per_image(), TH_LAST, TH_LOC, gross_px=8.0, depth=maps)
+    assert _bits(o["ur"][:rows], uR)
+    assert nm0.min() > 80 and nm2.min() > 100, (nm0, nm2)
+    assert checked["released"] >= 3 and checked["skipped"] > 100 and checked["in_view"] > 400 and checked["local"] > 200, checked
+    assert checked["stereo"] > 100, checked          # stereo edges wherever the map has a depth
     ex.close()
 
 
@@ -415,32 +304,6 @@ def test_rgbd_graph_replay_equals_eager_calls():
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-def _run(step, imgs, P, hl, hc, depth=None):
-    rc = len(imgs) * 1400
-    o = _outputs(len(imgs), rc, int(hc["off"][-1]))
-    step.submit(imgs, last=hl, local=hc, pose=hl["Tcw"], local_world_pos=hc["xw"], depth=depth)
-    rows = step.collect(o)
-    return rows, o
-
-
-def _same(a, b, stereo=False):
-    """two steps' results are identical; a stereo step's right-eye rows of uright / depth are unused (not written) and not compared"""
-    rows_a, oa = a
-    rows_b, ob = b
-    assert rows_a == rows_b
-    rows = np.arange(rows_a)
-    if stereo:
-        off = oa["offsets"]
-        rows = np.concatenate([np.arange(off[2 * p], off[2 * p + 1]) for p in range(len(off) // 2)])
-    for key in oa:
-        x, y = oa[key], ob[key]
-        if key in ("kps", "desc", "fm"):
-            x, y = x[:rows_a], y[:rows_a]
-        elif key in ("ur", "dep"):
-            x, y = x[rows], y[rows]
-        assert (x.view(np.uint8) == y.view(np.uint8)).all(), key
-
-
 def _setup(P, seed):
     g = GEOM["tum_640x480"]
     W, H, NF, FX, FY, CX, CY, BF = g
@@ -491,12 +354,12 @@ def test_rgbd_refusals_leave_the_handle_usable():
                  (P, dp, 1, 2 * W, 2 * W * H - 2), (P, dp, 2, 2 * W, 2 * W * H), (P, None, 1, 2 * W, 2 * W * H)]:
         assert L.orbm_stereo_rgbd_batch(h, args[0], args[1], args[2], args[3], args[4], float(FACTOR), 0, float(BF)) == ORB_ERR_INVALID, args
     # the same handle then runs a correct RGB-D step and a correct stereo step; each equals a fresh handle's
-    got = _run(rgbd, imgs, P, hl, hc, maps)
-    _same(got, _run(mk(fresh, "rgbd"), imgs, P, hl, hc, maps))
+    got = run_step(rgbd, imgs, hl, hc, depth=maps)
+    same_results(got, run_step(mk(fresh, "rgbd"), imgs, hl, hc, depth=maps))
     assert (got[1]["dep"][:got[0]] > 0).sum() > 1000 and got[1]["nm1"].min() > 50
-    got = _run(mk(ex, "stereo"), stereo_imgs, P, sl, sc)
+    got = run_step(mk(ex, "stereo"), stereo_imgs, sl, sc)
     fresh2 = _mk(W, H, NF, 2 * P)
-    _same(got, _run(mk(fresh2, "stereo"), stereo_imgs, P, sl, sc), stereo=True)
+    same_results(got, run_step(mk(fresh2, "stereo"), stereo_imgs, sl, sc), stereo=True)
     for e in (ex, fresh, fresh2):
         e.close()
 
@@ -506,20 +369,22 @@ def test_no_state_leaks_between_stereo_monocular_and_rgbd_steps():
     g, imgs, maps, stereo_imgs, hl, hc, sl, sc, ml, mk = _setup(P, 2800)
     W, H, NF = g[:3]
     used = _mk(W, H, NF, 2 * P)
-    fresh = lambda: _mk(W, H, NF, 2 * P)
-    runs = {"stereo": lambda e: _run(mk(e, "stereo"), stereo_imgs, P, sl, sc), "mono": lambda e: _run(mk(e, "mono"), imgs, P, ml, hc),
-            "rgbd": lambda e: _run(mk(e, "rgbd"), imgs, P, hl, hc, maps)}
-    want = {}
-    for kind in runs:
-        f = fresh()
-        want[kind] = runs[kind](f)
-        f.close()
-    for kind in ["stereo", "rgbd", "mono", "rgbd", "stereo", "mono", "stereo"]:     # every ordered pair of the three sensors
-        _same(runs[kind](used), want[kind], stereo=kind == "stereo")
-    rows, o = want["mono"]
-    assert (o["ur"][:rows] == -1).all() and (o["dep"][:rows] == -1).all()          # monocular after RGB-D still reports -1
-    rows, o = want["rgbd"]
-    assert (o["ur"][:rows] > 0).sum() > 1000
+    for with_po in (False, True):
+        runs = {"stereo": lambda e: run_step(mk(e, "stereo"), stereo_imgs, sl, sc, with_po),
+                "mono": lambda e: run_step(mk(e, "mono"), imgs, ml, hc, with_po), "rgbd": lambda e: run_step(mk(e, "rgbd"), imgs, hl, hc, with_po, maps)}
+        want = {}
+        for kind in runs:
+            f = _mk(W, H, NF, 2 * P)
+            want[kind] = runs[kind](f)
+            f.close()
+        for kind in ["stereo", "rgbd", "mono", "rgbd", "stereo", "mono", "stereo"]:     # every ordered pair of the three sensors
+            same_results(runs[kind](used), want[kind], stereo=kind == "stereo")
+        rows, o = want["stereo"]
+        assert (o["ur"][:rows] > 0).sum() > 500, with_po                                 # the stereo step has real mvuRight values
+        rows, o = want["mono"]
+        assert (o["ur"][:rows] == -1).all() and (o["dep"][:rows] == -1).all(), with_po   # monocular after RGB-D still reports -1
+        rows, o = want["rgbd"]
+        assert (o["ur"][:rows] > 0).sum() > 1000, with_po
     used.close()
 
 
