@@ -181,6 +181,17 @@ LIBA_HD double liba_huber(double e, double delta, double dsqr, double* w) {
     return 2 * s * delta - dsqr;
 }
 
+// float32 a . b with every product and sum rounded on its own, as the reference's Eigen float arithmetic and the oracle round them
+// (DESIGN.md §2: float32 without FMA contraction).  Written with plain operators, nvcc fuses them into FFMA, which rounds once: the
+// bias-corrected preintegrated deltas then differ by a float ulp from the reference's, and so do the inertial residuals built on them.
+LIBA_HD float liba_fdot3(const float* a, const float* b) {
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(__fadd_rn(__fmul_rn(a[0], b[0]), __fmul_rn(a[1], b[1])), __fmul_rn(a[2], b[2]));
+#else
+    return a[0] * b[0] + a[1] * b[1] + a[2] * b[2];      // host builds of this file use -ffp-contract=off
+#endif
+}
+
 // team-wide sum / max in a fixed order (warp tree, warps in order, CTAs in rank order): every thread receives the same value
 LIBA_HD double liba_sum(const LibaDev& P, double v) {
 #if defined(__CUDA_ARCH__)
@@ -288,7 +299,7 @@ LIBA_HD void liba_inertial(const LibaDev& P, const LibaLink& L, double* e9, doub
     const double g[3] = {0, 0, -(double)9.81f};
     float dbg[3], dba[3], wv[3];
     for (int i = 0; i < 3; ++i) { dba[i] = (float)s1[18 + i] - L.bias[i]; dbg[i] = (float)s1[15 + i] - L.bias[3 + i]; }
-    for (int i = 0; i < 3; ++i) wv[i] = L.JRg[3 * i] * dbg[0] + L.JRg[3 * i + 1] * dbg[1] + L.JRg[3 * i + 2] * dbg[2];
+    for (int i = 0; i < 3; ++i) wv[i] = liba_fdot3(L.JRg + 3 * i, dbg);
     const double wd[3] = {wv[0], wv[1], wv[2]};
     double E[9], dR[9], dV[3], dP[3];
     so3_exp(wd, E);
@@ -296,10 +307,8 @@ LIBA_HD void liba_inertial(const LibaDev& P, const LibaLink& L, double* e9, doub
         for (int j = 0; j < 3; ++j)
             dR[3 * i + j] = (double)(float)((double)L.dR[3 * i] * E[j] + (double)L.dR[3 * i + 1] * E[3 + j] + (double)L.dR[3 * i + 2] * E[6 + j]);
     for (int i = 0; i < 3; ++i) {
-        dV[i] = (double)(float)(L.dV[i] + (L.JVg[3 * i] * dbg[0] + L.JVg[3 * i + 1] * dbg[1] + L.JVg[3 * i + 2] * dbg[2]) +
-                                (L.JVa[3 * i] * dba[0] + L.JVa[3 * i + 1] * dba[1] + L.JVa[3 * i + 2] * dba[2]));
-        dP[i] = (double)(float)(L.dP[i] + (L.JPg[3 * i] * dbg[0] + L.JPg[3 * i + 1] * dbg[1] + L.JPg[3 * i + 2] * dbg[2]) +
-                                (L.JPa[3 * i] * dba[0] + L.JPa[3 * i + 1] * dba[1] + L.JPa[3 * i + 2] * dba[2]));
+        dV[i] = (double)(L.dV[i] + liba_fdot3(L.JVg + 3 * i, dbg) + liba_fdot3(L.JVa + 3 * i, dba));
+        dP[i] = (double)(L.dP[i] + liba_fdot3(L.JPg + 3 * i, dbg) + liba_fdot3(L.JPa + 3 * i, dba));
     }
     double Rbw1[9], dRt[9], t1[9], eR[9], er[3];
     m3_T(s1, Rbw1);

@@ -209,7 +209,7 @@ orb_status __wrap_liba_solve(liba_handle* h, int32_t n_problems, const liba_prob
     if (s == ORB_OK) {
         r.put("state_out", R.state, 168 * (size_t)P.n_kf); r.put("point_out", R.point, 24 * (size_t)P.n_mp);
         r.put("edge_chi2", R.edge_chi2, 8 * (size_t)P.n_edges); r.put("edge_depth_positive", R.edge_depth_positive, P.n_edges);
-        const double st[5] = {(double)R.iterations, (double)R.trials, R.lambda, R.chi2, R.chi2_initial};
+        const double st[6] = {(double)R.iterations, (double)R.trials, R.lambda, R.chi2, R.chi2_initial, R.chi2_last_trial};
         r.put("stats", st, sizeof(st));
     }
     return s;

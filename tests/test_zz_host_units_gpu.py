@@ -715,6 +715,13 @@ def test_local_inertial_ba(tmp_path, name):
     assert scal[6] == (1e-2 if c.get("large") else 1.0) and int(scal[7]) == (4 if c.get("large") else 10)
     if not failed:                                             # a NaN window: nothing to compare but the failure rule below
         check(got, ref)
+        # what the outlier pass and the failure rule read, held to the oracle (the erasures below are restated from the record)
+        assert np.allclose(rc("edge_chi2", np.float64), ref["edge_chi2"], rtol=1e-6, atol=1e-8)
+        assert (rc("edge_depth_positive", np.uint8) == ref["edge_depth_pos"]).all()
+        assert abs(st[4] - ref["chi2_init"]) <= 1e-9 * max(1.0, ref["chi2_init"])
+        assert abs(st[5] - ref["chi2_last"]) <= 1e-6 * max(1.0, ref["chi2_last"])
+    fails = lambda c0, c1: bool(2 * np.float32(c0) < np.float32(c1) or np.isnan(c0) or np.isnan(c1))     # :2729-2735
+    assert fails(st[4], st[5]) == fails(ref["chi2_init"], ref["chi2_last"])
     # (b) the links the unit built: EdgeInertial's information from the keyframe's preintegration (inverse of C's 9 x 9 block, symmetrised),
     # scaled by 1e-2 and made robust on the oldest link of the window (Optimizer.cc:2467-2479), robust on every link with bRecInit
     st0 = rc("state", np.float64).reshape(nK, 21)
